@@ -3,7 +3,7 @@
     python bench.py [--gpus N] [--steps K] [--warmup W] [--workload c2|c3|c4] [--regime peaky|diffuse]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
     python bench.py --impl reference ...        # CPU arm: the unmodified Python reference over a fork pool
-                                                # (baseline/_ref; LM workloads: the oracle C++ port)
+                                                # (oracle/_ref; LM workloads: the oracle C++ port)
 
 A "step" is one decode_batch() pass over one batch of synthetic logits.  `value` is frames/s
 with the batch already resident in HBM (device pointers handed to the C ABI); `e2e` is the same
@@ -42,7 +42,7 @@ WORKLOADS = {
     "c3": dict(kind="char", vocab="B", n_words=20000, lm_order=3, T=1000, batch=1024, beam=100,
                lm=dict(alpha=0.5, beta=1.0), hot=0,
                name="Wav2Vec2-base V=32, T=1000, beam=100 + synthetic 3-gram (alpha=0.5,beta=1.0), batch=1024 per GPU"),
-    # opt-in (--secondary c3_biglm): the C3 shape with a ~10^7 n-gram model, i.e. tables several times the 126 MB L2
+    # opt-in (--secondary c3_biglm): the C3 shape with a ~10^7 n-gram model, i.e. tables several times the 50 MB L2 of an H100
     "c3_biglm": dict(kind="char", vocab="B", n_words=420000, lm_order=3, T=1000, batch=1024, beam=100,
                      lm=dict(alpha=0.5, beta=1.0), hot=0,
                      name="C3 shape + synthetic 3-gram over 420k words (~10^7 n-grams: tables several times the L2), batch=1024 per GPU"),
@@ -59,9 +59,9 @@ def make_workload(spec):
 
 
 class ClockSampler:
-    """SM clock and throttle reasons during the timed region (B200_PROFILING.md's clocks line), read through NVML
+    """SM clock and throttle reasons during the timed region, read through NVML
     in this process every 20 ms.  (A polling `nvidia-smi -lms` child process was used first: its driver queries
-    delayed the decode calls of the timed loop by up to 2 ms per step.)  Falls back to nvidia-smi without pynvml."""
+    delayed the decode calls of the timed loop.)  Falls back to nvidia-smi without pynvml."""
 
     FIELDS = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
               "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -150,8 +150,8 @@ class ClockSampler:
 
 def host_cores():
     """CPU threads this process can really use: os.cpu_count() capped by the scheduler affinity and by the
-    cgroup CPU quota (the GPU boxes report 128 logical CPUs under a 16-CPU quota; 128 runnable threads on
-    16 CPUs' worth of time only thrash -- measured 56 k frames/s against 83 k with 16-32 threads)."""
+    cgroup CPU quota (a container may report far more logical CPUs than its quota grants; that many runnable
+    threads on a few CPUs' worth of time only thrash)."""
     n = os.cpu_count() or 1
     try:
         n = min(n, len(os.sched_getaffinity(0)))
@@ -186,7 +186,7 @@ def workload_objects(spec):
 
 
 def config_of(spec, regime, beam, B, V, logits_dtype, world):
-    """the `config` object of a JSON line -- the SAME dict for the B200 arm and the reference arm"""
+    """the `config` object of a JSON line -- the SAME dict for the CUDA arm and the reference arm"""
     return {"workload": spec["name"], "regime": regime, "beam_width": beam, "batch_per_gpu": B, "T": spec["T"], "V": V,
             "logits_dtype": logits_dtype, "l2": "flushed between timed steps (512 MiB write)",
             "parallelism": "utterance-sharded x%d" % world}
@@ -221,11 +221,11 @@ def port_arm(wl, spec, kw, xs, beam, hot, target_cpu_seconds=20.0, min_utts=0, w
                       "%d threads, %.1f s" % (n, spec["T"], cores, dt)}, texts, n
 
 
-REF_DIR = os.path.join(ROOT, "baseline", "_ref")
+REF_DIR = os.path.join(ROOT, "oracle", "_ref")
 
 
 def pyref_available(spec):
-    """The unmodified reference (pip-installed from /root/reference into baseline/_ref, which travels to the GPU box)
+    """The unmodified reference (pip-installed into oracle/_ref by build(), see oracle.install_reference)
     can be timed for workloads without a language model: its only missing hard dependency is then pygtrie's import,
     served by the stand-in under oracle/refshim.  LM workloads would run on the pure-Python kenlm stand-in, which
     would handicap the reference -- they are timed on the C++ port instead."""
@@ -288,7 +288,7 @@ def reference_main(args, spec, B, beam):
                 vals.append(n * T / dt)
         ref.close()
         kind = "reference"
-        what = ("%d utterances x T=%d of the same workload, the UNMODIFIED Python reference (baseline/_ref, pyctcdecode 0.6.0) "
+        what = ("%d utterances x T=%d of the same workload, the UNMODIFIED Python reference (oracle/_ref, pyctcdecode 0.6.0) "
                 "through decode_batch over a fork Pool(%d), %.1f s per step" % (n, T, cores, n * T / vals[-1]))
     else:
         vals, info = [], None
@@ -317,7 +317,7 @@ def reference_main(args, spec, B, beam):
 
 
 def pyref_subprocess(args_workload, regime, beam, seconds):
-    """cpu_baseline of the B200 arm, `kind: reference`: the reference arm in a child process (the fork pool must not
+    """cpu_baseline of the CUDA arm, `kind: reference`: the reference arm in a child process (the fork pool must not
     be forked from a process that holds a CUDA context and helper threads)."""
     cmd = [sys.executable, os.path.abspath(__file__), "--impl", "reference", "--steps", "1", "--warmup", "0", "--workload",
            args_workload, "--regime", regime, "--beam", str(beam), "--emit-texts", "--ref-seconds", str(seconds)]
@@ -378,6 +378,9 @@ class Stepper:
         return total, tms, out
 
 
+H100_HBM_GBS = 3350.0          # NVIDIA H100 SXM data sheet (HBM3, 700 W card): the fallback when no measured peak exists
+
+
 def load_peaks():
     try:
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as fh:
@@ -400,7 +403,7 @@ def secondary_entry(torch, pkg, flush, name, spec, regime, beam, logits_dtype, c
     e2e_total, e2e_tms, out_e2e = st.timed(st.step_host, steps, warmup, flush)
     same = out == out_e2e
     frames = B * T
-    peak = float(load_peaks().get("hbm_gbs", 6650.0))
+    peak = float(load_peaks().get("hbm_gbs", H100_HBM_GBS))
     esz = 2 if logits_dtype == "f16" else 4
     ms_beam = statistics.mean(t["ms_beam"] for t in tms)
     ms_prep = statistics.mean(t["ms_prepare"] for t in tms)
@@ -461,7 +464,7 @@ def streaming_entry(torch, pkg, name, spec, n_streams, chunk=50, beam=100):
     informational: every chunk ends with _finalize_beams (sort, trim, prune), so the reference's own streaming result
     differs from its one-shot decode on a few percent of the utterances too; parity of the streaming path is what the
     22 reference-generated streaming goldens and `cpu_baseline.final_text_equals_b200` check.  CPU figure: the unmodified Python reference's own partial_decode_beams on
-    one stream (workloads without a language model, when baseline/_ref is present)."""
+    one stream (workloads without a language model, when oracle/_ref is present)."""
     t_start = time.perf_counter()
     wl, kw, _ = workload_objects(spec)
     T = spec["T"]
@@ -530,6 +533,7 @@ def strong_scaling(torch, dist, pkg, sharding, flush, rank, world, local_rank, s
     sharded()
     sharded()                                               # warm-up: buffers, kernel variant hint
     t_sh, texts = timed(sharded, steps)
+    resident = torch.cuda.get_device_properties(local_rank).multi_processor_count * 4    # 4 CTAs per SM at beam 100
     # the same list on ONE GPU through the same public call (rank 0 decodes, the others wait at the barrier)
     single_texts, t_single = None, None
     if rank == 0:
@@ -559,7 +563,36 @@ def strong_scaling(torch, dist, pkg, sharding, flush, rank, world, local_rank, s
             "speedup_vs_one_gpu": t_single / t_sh,
             "sharded_equals_single": bool(texts == single_texts), "steps": steps,
             "limit": "per-rank host work (Python list handling, per-utterance H2D copies) and the latency of one resident wave: "
-                     "%d utterances per GPU are %s the resident set" % (n_utts // world, "within" if n_utts // world <= 592 else "above")}
+                     "%d utterances per GPU are %s the resident set" % (n_utts // world, "within" if n_utts // world <= resident else "above")}
+
+
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(directory, out, call):
+    """--dump-outputs: what the timed call returned in its last step, as float64 .npy files, so that two builds can be
+    compared output for output.  Every returned text as Unicode code points (text_codepoints, cut by text_lengths),
+    n_texts per utterance (1 for decode_batch, the beam count for decode_beams_batch) and, for decode_beams_batch,
+    every beam's logit_score and lm_score.  Above 64 MB in all a fixed, seeded sample of the utterances is written,
+    their indices in utterance_index."""
+    per_utt = [[o] for o in out] if call == "decode_batch" else [[b.text for b in beams] for beams in out]
+    scores = None if call == "decode_batch" else [[(b.logit_score, b.lm_score) for b in beams] for beams in out]
+    idx = np.arange(len(per_utt))
+    size = 8 * sum(len(t) + 4 for texts in per_utt for t in texts)
+    if size > DUMP_LIMIT_BYTES:
+        keep = max(1, int(len(idx) * DUMP_LIMIT_BYTES / size))
+        idx = np.sort(np.random.default_rng(0).choice(len(idx), size=keep, replace=False))
+    texts = [t for i in idx for t in per_utt[i]]
+    arrays = {"utterance_index": idx.astype(np.float64),
+              "n_texts": np.array([len(per_utt[i]) for i in idx], np.float64),
+              "text_lengths": np.array([len(t) for t in texts], np.float64),
+              "text_codepoints": np.array([ord(c) for t in texts for c in t], np.float64)}
+    if scores is not None:
+        flat = np.array([sc for i in idx for sc in scores[i]], np.float64).reshape(-1, 2)
+        arrays.update(logit_score=flat[:, 0].copy(), lm_score=flat[:, 1].copy())
+    os.makedirs(directory, exist_ok=True)
+    for name, arr in arrays.items():
+        np.save(os.path.join(directory, name + ".npy"), arr)
 
 
 _REAL_STDOUT = None
@@ -601,7 +634,11 @@ def main():
     ap.add_argument("--ref-port", action="store_true", help="reference arm: time the oracle C++ port even where the Python reference can run")
     ap.add_argument("--ref-seconds", type=float, default=0.0, help="reference arm: target seconds of one step (default: sized from --steps)")
     ap.add_argument("--emit-texts", action="store_true", help="reference arm: add the transcripts of the last step to the JSON line")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write what the last timed step returned to DIR/<name>.npy (float64; see dump_outputs)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     args.warmup = max(args.warmup, 3) if args.impl == "b200" else args.warmup
 
     rank = int(os.environ.get("RANK", "0"))
@@ -621,7 +658,7 @@ def main():
         return reference_main(args, spec, B, beam)
 
     # ------------------------------------------------------------------------------------
-    # B200 arm
+    # CUDA arm
     # ------------------------------------------------------------------------------------
     import torch
 
@@ -639,7 +676,7 @@ def main():
         torch.cuda.set_device(local_rank)
     import pyctcdecode_b200 as pkg
     from pyctcdecode_b200 import sharding
-    if os.environ.get("B200CTC_PROFILING_LIB"):   # opt-in phase-clock build (profiles/README.md), never the default
+    if os.environ.get("B200CTC_PROFILING_LIB"):   # opt-in phase-clock build (-DB2C_PHASE_CLOCKS), never the default
         from pyctcdecode_b200 import _lib
         _lib.use_library(os.environ["B200CTC_PROFILING_LIB"])
 
@@ -665,6 +702,8 @@ def main():
     clocks = sampler.stop() if rank == 0 else None
     e2e_total, e2e_tms, texts_e2e = st.timed(st.step_host, args.steps, args.warmup, flush)   # the same W warm-up steps as the device-resident arm
     assert texts == texts_e2e
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, texts, args.call)
     if args.call != "decode_batch":
         texts = [beams[0].text if beams else "" for beams in texts]
 
@@ -683,15 +722,9 @@ def main():
     ms_beam = statistics.mean(t["ms_beam"] for t in tms)
     ms_prep = statistics.mean(t["ms_prepare"] for t in tms)
     peaks = load_peaks()
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak = float(peaks.get("hbm_gbs", H100_HBM_GBS))
     esz = 2 if args.logits_dtype == "f16" else 4      # algorithmic bytes per logit: the dtype the rows arrive in
     alg_bytes = frames_per_step * wl.V * esz
-    traffic = None
-    try:
-        with open(os.path.join(ROOT, "profiles", "ncu_traffic.json")) as fh:
-            traffic = json.load(fh).get(args.workload, {}).get("beam_kernel_dram_bytes")
-    except OSError:
-        pass
     ach = alg_bytes / (ms_beam * 1e-3) / 1e9
     ach_prep = alg_bytes / (ms_prep * 1e-3) / 1e9 if ms_prep > 0 else None
     out = {
@@ -700,7 +733,7 @@ def main():
         "dtype": "f64", "data": "synthetic",
         "config": config_of(spec, args.regime, beam, B, wl.V, args.logits_dtype, world),
         "roofline": {"bound": "hbm", "kernel": "b2c_beam_kernel", "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak,
-                     "traffic": traffic, "peak_source": "MEASURED_PEAKS.json hbm_gbs (of measured)" if peaks else "fallback 6.65 TB/s (of fallback)",
+                     "peak_source": "MEASURED_PEAKS.json hbm_gbs (of measured)" if peaks else "H100 SXM data sheet, 3.35 TB/s (not measured)",
                      "algorithmic_bytes_per_launch": alg_bytes, "kernel_ms": ms_beam,
                      "note": "the beam kernel is a T-step serial chain per utterance (latency bound); the streaming stage is reported under roofline_prepare"},
         "roofline_prepare": {"bound": "hbm", "kernel": "b2c_prepare_kernel", "achieved": ach_prep, "peak": peak, "unit": "GB/s",

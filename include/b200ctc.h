@@ -1,4 +1,4 @@
-/* b200ctc.h -- C ABI of libb200ctc.so, the B200-native CTC prefix beam-search decoder.
+/* b200ctc.h -- C ABI of libb200ctc.so, the CUDA-native (H100, sm_90a) CTC prefix beam-search decoder.
  *
  * The reference (kensho-technologies/pyctcdecode 0.6.0) has no FFI: its "plugin API" for
  * this path is the Python class BeamSearchDecoderCTC.  This header is the boundary a

@@ -1,7 +1,7 @@
-"""TEST INFRASTRUCTURE ONLY (build container only: needs /root/reference).
+"""TEST INFRASTRUCTURE ONLY (needs a checkout of the reference: $PYCTCDECODE_REFERENCE or ../reference).
 
 Differential check of the C++ oracle (oracle/ctc_oracle.cpp) against the UNMODIFIED reference
-imported from /root/reference with the stand-ins in oracle/refshim.  Run:
+imported from that checkout with the stand-ins in oracle/refshim.  Run:
     python oracle/check_vs_reference.py [n_random]
 Prints one line per case family and exits non-zero on any mismatch that is neither
   (a) a permutation inside a group of beams the reference itself separates by <= `tie` in lm_score
@@ -20,8 +20,9 @@ import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
+REF = os.environ.get("PYCTCDECODE_REFERENCE") or os.path.join(ROOT, os.pardir, "reference")   # the reference checkout
 sys.path.insert(0, os.path.join(HERE, "refshim"))
-sys.path.insert(0, "/root/reference")
+sys.path.insert(0, REF)
 sys.path.insert(0, ROOT)
 
 import logging  # noqa: E402
@@ -103,7 +104,7 @@ def compare(ref_beams, orc_beams, tag, stats, ref_dec=None, x=None, dkw=None):
 def main():
     n_random = int(sys.argv[1]) if len(sys.argv) > 1 else 40
     stats = {"n": 0, "mismatch": []}
-    ref_tests = "/root/reference/pyctcdecode/tests"
+    ref_tests = os.path.join(REF, "pyctcdecode", "tests")
     arpa = os.path.join(ref_tests, "sample_data", "bugs_bunny_kenlm.arpa")
 
     # ---- the reference's own fixtures -------------------------------------------------

@@ -1,9 +1,9 @@
-"""TEST INFRASTRUCTURE ONLY (build container only: needs /root/reference).
+"""TEST INFRASTRUCTURE ONLY (needs a checkout of the reference: $PYCTCDECODE_REFERENCE or ../reference).
 
 Generates tests/golden/{cases.json,arrays.npz} by running the UNMODIFIED reference
-(/root/reference/pyctcdecode, imported with the kenlm / pygtrie stand-ins of oracle/refshim)
+(pyctcdecode/ of that checkout, imported with the kenlm / pygtrie stand-ins of oracle/refshim)
 on (a) the reference's own test fixtures (tests/test_decoder.py:186-223, sample_data/) and
-(b) small seeded synthetic utterances (tests/synth.py).  The GPU box has no /root/reference,
+(b) small seeded synthetic utterances (tests/synth.py).  The GPU machines need no reference checkout,
 so the parity tests read these committed vectors instead.
 
     python oracle/gen_golden.py
@@ -16,8 +16,9 @@ import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
+REF = os.environ.get("PYCTCDECODE_REFERENCE") or os.path.join(ROOT, os.pardir, "reference")   # the reference checkout
 sys.path.insert(0, os.path.join(HERE, "refshim"))
-sys.path.insert(0, "/root/reference")
+sys.path.insert(0, REF)
 sys.path.insert(0, ROOT)
 
 import logging  # noqa: E402
@@ -29,7 +30,7 @@ from pyctcdecode.alphabet import Alphabet  # noqa: E402
 
 from tests import synth  # noqa: E402
 
-REF_TESTS = "/root/reference/pyctcdecode/tests"
+REF_TESTS = os.path.join(REF, "pyctcdecode", "tests")
 OUT = os.path.join(ROOT, "tests", "golden")
 
 

@@ -1,4 +1,4 @@
-"""TEST INFRASTRUCTURE ONLY (build container only: needs /root/reference).
+"""TEST INFRASTRUCTURE ONLY (needs a checkout of the reference: $PYCTCDECODE_REFERENCE or ../reference).
 
 MultiLanguageModel goldens: the UNMODIFIED reference's BeamSearchDecoderCTC over a MultiLanguageModel
 (language_model.py:455-502; its own test: tests/test_decoder.py:386-401) on seeded inputs
@@ -14,8 +14,9 @@ import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
+REF = os.environ.get("PYCTCDECODE_REFERENCE") or os.path.join(ROOT, os.pardir, "reference")   # the reference checkout
 sys.path.insert(0, os.path.join(HERE, "refshim"))
-sys.path.insert(0, "/root/reference")
+sys.path.insert(0, REF)
 sys.path.insert(0, ROOT)
 
 import logging  # noqa: E402
@@ -29,7 +30,7 @@ from pyctcdecode.alphabet import Alphabet  # noqa: E402
 
 from tests import synth  # noqa: E402
 
-REF_TESTS = "/root/reference/pyctcdecode/tests"
+REF_TESTS = os.path.join(REF, "pyctcdecode", "tests")
 OUT = os.path.join(ROOT, "tests", "golden")
 
 

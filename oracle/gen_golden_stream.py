@@ -1,9 +1,9 @@
-"""TEST INFRASTRUCTURE ONLY (build container only: needs /root/reference).
+"""TEST INFRASTRUCTURE ONLY (needs a checkout of the reference: $PYCTCDECODE_REFERENCE or ../reference).
 
 Streaming goldens: runs the UNMODIFIED reference's get_starting_state / partial_decode_beams
 (decoder.py:669-728, exercised by its tests/test_decoder.py:515-698) chunk by chunk and records
 the LMBeam list every call returns -> tests/golden/stream_cases.json (+ stream_arrays.npz for
-inputs that are not in arrays.npz).  The GPU box has no /root/reference; the parity tests read
+inputs that are not in arrays.npz).  The GPU machines need no reference checkout; the parity tests read
 these committed vectors.
 
     python oracle/gen_golden_stream.py
@@ -16,8 +16,9 @@ import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
+REF = os.environ.get("PYCTCDECODE_REFERENCE") or os.path.join(ROOT, os.pardir, "reference")   # the reference checkout
 sys.path.insert(0, os.path.join(HERE, "refshim"))
-sys.path.insert(0, "/root/reference")
+sys.path.insert(0, REF)
 sys.path.insert(0, ROOT)
 
 import logging  # noqa: E402
@@ -29,7 +30,7 @@ from pyctcdecode.language_model import HotwordScorer  # noqa: E402
 
 from tests import synth  # noqa: E402
 
-REF_TESTS = "/root/reference/pyctcdecode/tests"
+REF_TESTS = os.path.join(REF, "pyctcdecode", "tests")
 OUT = os.path.join(ROOT, "tests", "golden")
 
 

@@ -1,4 +1,4 @@
-"""TEST INFRASTRUCTURE ONLY (build container only: needs /root/reference).
+"""TEST INFRASTRUCTURE ONLY (needs a checkout of the reference: $PYCTCDECODE_REFERENCE or ../reference).
 
 Golden vectors for cases whose reference output is decided by rounding noise.  LibriSpeech logits of the
 reference's test data are INTEGER valued, so with wide settings (beam_prune_logp=-20, token_min_logp=-8) many beams
@@ -23,8 +23,9 @@ import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
+REF = os.environ.get("PYCTCDECODE_REFERENCE") or os.path.join(ROOT, os.pardir, "reference")   # the reference checkout
 sys.path.insert(0, os.path.join(HERE, "refshim"))
-sys.path.insert(0, "/root/reference")
+sys.path.insert(0, REF)
 sys.path.insert(0, ROOT)
 
 import logging  # noqa: E402
@@ -35,7 +36,7 @@ from pyctcdecode import build_ctcdecoder  # noqa: E402  (the reference)
 
 from tests import synth  # noqa: E402
 
-REF_TESTS = "/root/reference/pyctcdecode/tests"
+REF_TESTS = os.path.join(REF, "pyctcdecode", "tests")
 OUT = os.path.join(ROOT, "tests", "golden", "unstable_cases.json")
 N_PERTURB = 32
 EPS = 1e-13

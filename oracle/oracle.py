@@ -28,6 +28,29 @@ def build(force=False):
     return _LIB_PATH
 
 
+REF_DIR = os.path.join(_HERE, "_ref")
+
+
+def install_reference():
+    """oracle/_ref = the unmodified reference (pyctcdecode 0.6.0), pip-installed for bench.py's reference arm.  The
+    source checkout is $PYCTCDECODE_REFERENCE, or a `reference` directory next to this repository; without one nothing
+    is installed and the reference arm times the C++ port instead.  Installed from a copy: the checkout may be read-only."""
+    src = os.environ.get("PYCTCDECODE_REFERENCE") or os.path.join(os.path.dirname(_HERE), os.pardir, "reference")
+    if os.path.isdir(os.path.join(REF_DIR, "pyctcdecode")) or not os.path.isfile(os.path.join(src, "pyproject.toml")):
+        return
+    import shutil
+    import sys
+    import tempfile
+    with tempfile.TemporaryDirectory() as tmp:
+        copy = os.path.join(tmp, "reference")
+        shutil.copytree(src, copy, ignore=shutil.ignore_patterns(".git"))
+        cmd = [sys.executable, "-m", "pip", "install", "--no-index", "--no-build-isolation", "--no-deps", "--quiet",
+               "--target", REF_DIR, copy]
+        log = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
+        if log.returncode != 0:  # the reference arm then falls back to the C++ port and says so; not a build failure
+            print("oracle/_ref: pip install failed:\n" + log.stdout[-2000:], file=sys.stderr)
+
+
 def lib():
     global _lib
     if _lib is None:

@@ -1,6 +1,6 @@
 """ctypes binding of libb200ctc.so (C ABI declared in include/b200ctc.h).
 
-The shared library is built in-tree by ``__graft_entry__.build()`` (nvcc, sm_100a).  There is
+The shared library is built in-tree by ``__graft_entry__.build()`` (nvcc, sm_90a).  There is
 no CPU implementation: if the library is missing, or the machine has no CUDA device, every
 decode call raises -- loudly, by design.
 """

@@ -1,4 +1,4 @@
-"""Label normalisation for the B200 decoder.
+"""Label normalisation for the CUDA decoder.
 
 Host-side, O(V), build time only -- but it decides which token is the CTC blank, which one
 separates words and whether the alphabet is BPE, i.e. what the kernels are specialised on, so

@@ -1,5 +1,5 @@
 // b200ctc -- C ABI implementation (include/b200ctc.h): kernels, workspace layout, batch
-// orchestration, result assembly.  Compiled by nvcc for sm_100a into libb200ctc.so.
+// orchestration, result assembly.  Compiled by nvcc for sm_90a into libb200ctc.so.
 // With -DB2C_HOSTSIM (tests/hostsim only) the same file is compiled by g++ against a stub of
 // the CUDA runtime and runs the kernel bodies block by block on the CPU so that kernel logic
 // can be tested where there is no GPU; that build is never loaded by the product package.
@@ -1672,8 +1672,8 @@ static int decode_batch_locked(b2c_decoder_t* d, const void* const* logits, cons
         // its phases are loops over hundreds to thousands of candidates, each a chain of dependent memory accesses
         if (cls == kNumCaps && per_sm_of(ln.L.smem_bytes, 128) == 1) ln.threads = 256;
         // beam tables that do not fit shared memory (beam_width in the thousands) live in HBM: every phase is a chain of L2
-        // round trips, and twice the threads at half the registers hide more of them (measured at beam 2000 on the C2
-        // shape: 56 -> 49 ms; with the tables in shared memory, beam 500, the spills cost more than they hide: 19 -> 22 ms)
+        // round trips, and twice the threads at half the registers hide more of them (with the tables in shared memory,
+        // e.g. beam 500, the spills cost more than they hide)
         if (cls == kNumCaps && ln.threads == 256 && !ln.L.beams_in_smem) ln.threads = 512;
         ln.per_sm = per_sm_of(ln.L.smem_bytes, ln.threads);
         }
@@ -1730,8 +1730,7 @@ static int decode_batch_locked(b2c_decoder_t* d, const void* const* logits, cons
     }
     static const int force_chunks = std::getenv("B200CTC_FORCE_CHUNKS") ? std::atoi(std::getenv("B200CTC_FORCE_CHUNKS")) : 0;   // tests
     // Chunk boundaries.  A chunked launch ends when its SLOWEST utterance has finished the chunk, so every boundary
-    // costs the spread of the per-chunk times (measured: 4 equal chunks at C2 take 4.8 ms of beam kernel instead of
-    // 3.75).  Compute-bound calls (the copy is shorter than the decode) therefore use TWO chunks: a short first one whose
+    // costs the spread of the per-chunk times.  Compute-bound calls (the copy is shorter than the decode) therefore use TWO chunks: a short first one whose
     // decode covers the copy of the rest; copy-bound calls (large alphabets) use equal chunks.
     std::vector<int> bounds{0, std::max(T_max, 0)};
     // GATED launch (preferred for pipelined calls): ONE beam launch that starts after the first chunk and waits, on the
@@ -1739,12 +1738,12 @@ static int decode_batch_locked(b2c_decoder_t* d, const void* const* logits, cons
     // streaming stage of the later chunks runs CONCURRENTLY with the beam kernel on another stream, which needs free SM
     // resources: only taken when the beam kernel leaves at least n_sm/8 CTA slots empty; a CTA that waits longer than
     // ~40 ms gives up with B2C_ERR_GATE and the call is redone as a plain call.
-    // Which form of pipelining (measured on B200, profiles/pipeline_r02.txt):
-    //   compute-bound calls (copy < 0.6 x decode; C2: copy 0.6 ms, decode 3.9 ms) -> the gated launch: 5.05 -> 4.42 ms of
-    //     device time; chunked launches gain nothing there -- a chunked launch ends when its slowest utterance has finished
-    //     the chunk, so every boundary costs the spread of the per-chunk times;
-    //   copy-bound calls (C4 shape: copy 20 ms, decode 7 ms) -> chunked launches, equal chunks: 25.9 -> 20.8 ms (the gated
-    //     form is slower there, 22.8 ms: the streaming stage of a 1 GB batch crawls on the SM slots the beam kernel leaves free).
+    // Which form of pipelining:
+    //   compute-bound calls (copy < 0.6 x decode, e.g. C2) -> the gated launch; chunked launches gain nothing there -- a
+    //     chunked launch ends when its slowest utterance has finished the chunk, so every boundary costs the spread of
+    //     the per-chunk times;
+    //   copy-bound calls (e.g. the C4 shape) -> chunked launches, equal chunks (the gated form is slower there: the
+    //     streaming stage of a 1 GB batch crawls on the SM slots the beam kernel leaves free).
     // The plan of a pipelined call comes from the hint alone; it must be the plan the previous plain call of this
     // configuration ran (another kernel variant would change the speed, not the result: diffuse batches decode 35 % slower
     // on the latency-first kernel the hint-only plan picks than on the capacity-class kernel their statistics pick).

@@ -1,7 +1,7 @@
 // b200ctc -- latency-first variant of the per-utterance prefix beam search for beam_width <= WC
 // (same algorithm and the same results as b2c_beam.h, which stays the general path).
 //
-// A C2-shaped batch (256 utterances x 1000 frames on 148 SMs) keeps every utterance resident, so the
+// A C2-shaped batch (256 utterances x 1000 frames on the 132 SMs of an H100) keeps every utterance resident, so the
 // batch takes exactly as long as ONE utterance: T dependent frames.  What bounds it is the latency
 // of a frame, not throughput.  Compared with the general kernel this variant therefore
 //   * uses a compile-time shared-memory layout (B2cFastSmem): every array address is

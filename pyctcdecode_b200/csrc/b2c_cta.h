@@ -6,7 +6,7 @@
 //     B2C_SYNC();
 //     B2C_LEADER { ... one thread ... }
 //
-// Compiled by nvcc for sm_100a these are the obvious CUDA constructs.  Compiled by g++ with
+// Compiled by nvcc for sm_90a these are the obvious CUDA constructs.  Compiled by g++ with
 // B2C_HOSTSIM (tests/hostsim only -- NOT a product fallback, the product library contains no
 // CPU path) a phase is a plain loop over all items and a barrier is a no-op, i.e. one legal
 // interleaving of the CUDA execution.  Code outside B2C_FOR / B2C_LEADER between barriers

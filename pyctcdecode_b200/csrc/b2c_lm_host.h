@@ -1,6 +1,6 @@
 // b200ctc -- host side of the n-gram model: ARPA text -> flat, relocatable tables.
 //
-// B200-native replacement for what the reference gets from the third-party kenlm package
+// GPU-native replacement for what the reference gets from the third-party kenlm package
 // (kenlm.Model(path): reference decoder.py:1074, language_model.py:451) and from
 // pygtrie.CharTrie over the unigram list (language_model.py:263).  The result is ONE
 // contiguous blob (header + unigram array + n-gram hash table + vocabulary hash table +

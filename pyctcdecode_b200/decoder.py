@@ -1,5 +1,5 @@
 """BeamSearchDecoderCTC / build_ctcdecoder with the reference's call surface, dispatching the
-whole beam search to the sm_100a kernels through the C ABI (include/b200ctc.h).
+whole beam search to the sm_90a kernels through the C ABI (include/b200ctc.h).
 
 What stays on the host: argument checking (reference decoder.py:330-344), packaging the list
 of [T_i, V] matrices into one ``b2c_decode_batch`` call, turning results into ``OutputBeam``.

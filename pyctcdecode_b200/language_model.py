@@ -1,4 +1,4 @@
-"""Host-side language-model objects of the B200 decoder.
+"""Host-side language-model objects of the CUDA decoder.
 
 Same surface as reference pyctcdecode/language_model.py (LanguageModel, HotwordScorer, the
 state wrappers), but the n-gram engine is the library's own flattened model

@@ -2,7 +2,7 @@
 collective.
 
 The reference's only parallelism is ``multiprocessing.Pool.map`` over utterances with the LM
-shared by fork copy-on-write (reference decoder.py:895-945, :262-269).  The B200 equivalent:
+shared by fork copy-on-write (reference decoder.py:895-945, :262-269).  The GPU equivalent:
 every rank owns one GPU and a shard of the utterances; the flattened LM is built once (rank
 ``src`` parses the ARPA file) and shipped to the other ranks with ONE ``torch.distributed``
 broadcast (NCCL over NVLink on a GPU box, gloo in the CPU tests); after that ranks never talk

@@ -1,6 +1,6 @@
 // TEST INFRASTRUCTURE ONLY -- minimal stand-in for the CUDA runtime used by tests/hostsim.
 //
-// The product library (pyctcdecode_b200/csrc, built by nvcc for sm_100a) has NO CPU path.
+// The product library (pyctcdecode_b200/csrc, built by nvcc for sm_90a) has NO CPU path.
 // To be able to exercise the kernel *logic* (hashing, merge, LM fusion, selection, backtrack)
 // in the CPU-only CI container, tests/hostsim compiles the very same sources with g++ and
 // -DB2C_HOSTSIM: kernel bodies run block by block on the host (see csrc/b2c_cta.h) and the

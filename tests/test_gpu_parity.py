@@ -1,7 +1,7 @@
-"""GPU parity tests (`pytest -m gpu`, run on the B200 box): the CUDA path through the C ABI
+"""GPU parity tests (`pytest -m gpu`, run on an H100): the CUDA path through the C ABI
 against (a) the golden vectors generated from the unmodified reference, (b) the CPU oracle on
 seeded inputs at sizes the oracle finishes in seconds, (c) size-independent properties at
-BASELINE.json's full sizes.  Nothing here reads /root/reference.
+BASELINE.json's full sizes.  Nothing here reads the reference checkout.
 
 Tolerances: transcripts and word frames must be identical; beam scores within 1e-9 relative of
 the oracle (same float64 operation order; only CUDA's vs glibc's exp/log can differ in the
@@ -27,7 +27,7 @@ def pkg():
     L = _lib.lib()
     assert _lib.library_path() == _lib.DEFAULT_LIBRARY
     if L.b2c_device_count() < 1:
-        pytest.skip("no CUDA device on this machine (the GPU parity tests run on the B200 box)")
+        pytest.skip("no CUDA device on this machine (the GPU parity tests need one)")
     return pyctcdecode_b200
 
 

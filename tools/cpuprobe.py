@@ -1,5 +1,5 @@
 import time, sys, os
-sys.path.insert(0, os.environ.get("GRAFT_REPO_ROOT", "/root/repo"))
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from tests import synth
 from oracle import oracle as orc
 print("cpu_count", os.cpu_count(), "affinity", len(os.sched_getaffinity(0)))

@@ -1,6 +1,6 @@
-"""Summary of one ncu --set full capture as JSON (the numbers profiles/README.md and bench.py's roofline.traffic quote).
+"""Summary of one ncu --set full capture as JSON.
 
-    python tools/ncu_summary.py <report.ncu-rep> > profiles/<name>_summary.json
+    python tools/ncu_summary.py <report.ncu-rep> > <name>_summary.json
 """
 import csv
 import io

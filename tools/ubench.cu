@@ -1,5 +1,5 @@
-// micro-benchmarks of the instruction latencies the beam kernel's critical path is made of (B200, sm_100a)
-// build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/ubench tools/ubench.cu ; run: tools/ubench
+// micro-benchmarks of the instruction latencies the beam kernel's critical path is made of (H100, sm_90a)
+// build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/ubench tools/ubench.cu ; run: tools/ubench
 #include <cstdio>
 #include <cuda_runtime.h>
 typedef unsigned long long u64; typedef unsigned int u32;

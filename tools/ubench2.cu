@@ -1,4 +1,4 @@
-// does a CTA-scope fence / block barrier wait for outstanding global loads and stores?  (B200, sm_100a)
+// does a CTA-scope fence / block barrier wait for outstanding global loads and stores?  (H100, sm_90a)
 #include <cstdio>
 #include <cuda_runtime.h>
 typedef unsigned long long u64; typedef unsigned int u32;
