@@ -233,7 +233,7 @@ typedef struct {
     int launches;              /* kernels launched                                         */
     long long h2d_bytes, d2h_bytes;
     long long frames;          /* sum of T                                                 */
-    long long tokens;          /* selected (frame, token) pairs                            */
+    long long tokens;          /* (frame, token) pairs the streaming stage emitted          */
     int cap_candidates;        /* shared-memory candidate capacity class chosen for the call */
     int cta_threads;           /* threads per CTA of the beam kernel                        */
     int cta_slots;             /* resident CTAs (utterances in flight)                      */
@@ -246,6 +246,13 @@ typedef struct {
                                   waiting for this call's (no mid-call synchronisation); same results either way */
 } b2c_timings_t;
 int b2c_decoder_last_timings(const b2c_decoder_t* dec, b2c_timings_t* out);
+/* Diagnostics: the (token id, log-prob) lists the streaming stage wrote in the LAST call, as the beam kernel consumed
+ * them -- every frame's list in emission order, frame after frame, utterance after utterance.  With NULL arrays only
+ * the sizes are returned.  counts / rec_id0 / rec_lp0: [n_frames] (list length, and the first token and log-prob of
+ * the frame's record); ids / lps: [n_entries]; is_prob: one flag per utterance of the last call (1: the utterance was
+ * taken as probabilities). */
+int b2c_decoder_last_tokens(const b2c_decoder_t* dec, int64_t* n_frames, int64_t* n_entries, int32_t* counts, uint32_t* ids,
+                            double* lps, uint16_t* rec_id0, double* rec_lp0, int32_t* is_prob);
 
 #ifdef __cplusplus
 }

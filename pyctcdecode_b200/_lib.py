@@ -135,6 +135,7 @@ def _declare(L):
     L.b2c_result_frames.restype = C.POINTER(C.c_int32)
     L.b2c_result_lm_state.argtypes = [vp, i32, i32, C.POINTER(LMState)]
     L.b2c_decoder_last_timings.argtypes = [vp, C.POINTER(Timings)]
+    L.b2c_decoder_last_tokens.argtypes = [vp, C.POINTER(C.c_int64), C.POINTER(C.c_int64), vp, vp, vp, vp, vp, vp]
     L.b2c_decoder_add_lm.argtypes = [vp, vp]
     L.b2c_decoder_set_params_lm.argtypes = [vp, i32, f64, f64, f64, i32]
     L.b2c_result_lm_state_at.argtypes = [vp, i32, i32, i32, C.POINTER(LMState)]

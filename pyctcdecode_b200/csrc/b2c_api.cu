@@ -568,8 +568,9 @@ struct b2c_decoder {
     // statistics-based call of the configuration ran
     bool hinted_refused = false;          // the hint-only plan differed: plan from the statistics until the next refresh
     u32 hinted_calls = 0;                 // every 32nd call of a configuration plans from its statistics again (data may drift)
-    std::mutex call_mu;                   // b2c_decode_batch is serialised per handle (scratch buffers are per handle)
+    mutable std::mutex call_mu;           // b2c_decode_batch is serialised per handle (scratch buffers are per handle)
     b2c_timings_t tm;
+    std::vector<int32_t> last_T;          // frames per utterance of the last call that completed (b2c_decoder_last_tokens)
     // adaptive sizing: candidate-count histogram of the previous call with the same configuration
     bool hint_valid = false;
     int hint_beam = 0, hint_lm = 0, hint_hot = 0, hint_prune = 0;
@@ -1133,6 +1134,7 @@ static int decode_batch_locked(b2c_decoder_t* d, const void* const* logits, cons
     const int dtype_in = dtype;
     const bool half_in = dtype_in == B2C_DTYPE_F16 || dtype_in == B2C_DTYPE_BF16;
     if (half_in) dtype = B2C_DTYPE_F32;
+    d->last_T.clear();
     if (opts->beam_width < 1) return fail(B2C_E_ARG, "beam_width must be >= 1");
     if (opts->beam_width > 65535) return fail(B2C_E_ARG, "beam_width above 65535 is not supported");
     std::unique_ptr<b2c_result> res(new b2c_result());
@@ -1944,6 +1946,8 @@ static int decode_batch_locked(b2c_decoder_t* d, const void* const* logits, cons
     if (!text_only) CUDA_OK(cudaMemcpyAsync(d->h_out_frames.p, d->d_out_frames.p, frm_bytes, cudaMemcpyDeviceToHost, st));
     if (d->h_mstats.ensure(64)) return B2C_E_NOMEM;
     CUDA_OK(cudaMemcpyAsync(d->h_mstats.p, d->d_mstats.p, 64, cudaMemcpyDeviceToHost, st));
+    // selected-token totals (b2c_timings_t.tokens); a plain call already copied them for the launch plan
+    if (pipe_candidate) CUDA_OK(cudaMemcpyAsync(d->h_sumk.p, d->d_sumk.p, 4ull * n_utts, cudaMemcpyDeviceToHost, st));
     CUDA_OK(cudaEventRecord(d->ev[4], st));
     hp_mark(2);                                   // launch planning + enqueue of the beam kernel and D2H
     CUDA_OK(cudaStreamSynchronize(st));
@@ -2060,9 +2064,9 @@ static int decode_batch_locked(b2c_decoder_t* d, const void* const* logits, cons
     if (cudaEventElapsedTime(&ms, d->ev[0], d->ev[4]) == cudaSuccess) d->tm.ms_total = ms;
     d->tm.frames = static_cast<long long>(total_frames);
     d->last_device_ms = static_cast<double>(d->tm.ms_prepare) + static_cast<double>(d->tm.ms_beam);
-    // total selected tokens = last tok_start of the last utterance ... summed per utterance is not
-    // available without a reduction; report the last utterance's end offset only when B == 1
     d->tm.tokens = 0;
+    for (int i = 0; i < n_utts; ++i) d->tm.tokens += static_cast<long long>(d->h_sumk.as<u32>()[i]);
+    d->last_T.assign(T, T + n_utts);
 
     // ---- assemble results -------------------------------------------------------------------
     const int* h_nb = reinterpret_cast<const int*>(hs + off_nb);
@@ -2281,6 +2285,57 @@ int b2c_decoder_token_id(const b2c_decoder_t* d, const char* label) {
 int b2c_decoder_last_timings(const b2c_decoder_t* d, b2c_timings_t* out) {
     if (!d || !out) return fail(B2C_E_ARG, "null argument");
     *out = d->tm;
+    return 0;
+}
+// The streaming stage's output of the last call, read back from the decoder's buffers: frame t of utterance u has
+// rec.cnt entries at (frame_off[u] + (t & ~7)) * V + rec.off (offsets are relative to the frame's run of 8 frames).
+int b2c_decoder_last_tokens(const b2c_decoder_t* d, int64_t* n_frames, int64_t* n_entries, int32_t* counts, uint32_t* ids,
+                            double* lps, uint16_t* rec_id0, double* rec_lp0, int32_t* is_prob) {
+    if (!d || !n_frames || !n_entries) return fail(B2C_E_ARG, "null argument");
+    std::lock_guard<std::mutex> lk(d->call_mu);
+    const u64 V = static_cast<u64>(d->V);
+    u64 total = 0;
+    for (int32_t t : d->last_T) total += static_cast<u64>(t);
+    *n_frames = static_cast<int64_t>(total);
+    *n_entries = 0;
+    if (total == 0) {
+        if (is_prob) for (size_t u = 0; u < d->last_T.size(); ++u) is_prob[u] = 0;
+        return 0;
+    }
+    CUDA_OK(cudaSetDevice(d->device));
+    std::vector<B2cFrameRec> rec(total);
+    CUDA_OK(cudaMemcpyAsync(rec.data(), d->d_tok_start.p, sizeof(B2cFrameRec) * total, cudaMemcpyDeviceToHost, d->stream));
+    std::vector<int> isp(d->last_T.size());
+    CUDA_OK(cudaMemcpyAsync(isp.data(), d->d_isprob.p, 4 * isp.size(), cudaMemcpyDeviceToHost, d->stream));
+    const bool want_lists = ids || lps;
+    std::vector<u32> h_ids(want_lists ? total * V : 0);
+    std::vector<double> h_lp(want_lists ? total * V : 0);
+    if (want_lists) {
+        CUDA_OK(cudaMemcpyAsync(h_ids.data(), d->d_tok_ids.p, 4 * total * V, cudaMemcpyDeviceToHost, d->stream));
+        CUDA_OK(cudaMemcpyAsync(h_lp.data(), d->d_tok_lp.p, 8 * total * V, cudaMemcpyDeviceToHost, d->stream));
+    }
+    CUDA_OK(cudaStreamSynchronize(d->stream));
+    u64 f0 = 0, k = 0;
+    for (size_t u = 0; u < d->last_T.size(); ++u) {
+        const u64 Tn = static_cast<u64>(d->last_T[u]);
+        for (u64 t = 0; t < Tn; ++t) {
+            const B2cFrameRec& r = rec[f0 + t];
+            const u64 base = (f0 + (t & ~static_cast<u64>(B2C_RUN - 1))) * V + r.off;
+            if (r.cnt < 1 || r.cnt > V || base + r.cnt > total * V)
+                return fail(B2C_E_INTERNAL, "token list of a frame lies outside the token buffers");
+            if (counts) counts[f0 + t] = r.cnt;
+            if (rec_id0) rec_id0[f0 + t] = r.id0;
+            if (rec_lp0) rec_lp0[f0 + t] = r.lp0;
+            for (u64 q = 0; q < r.cnt && want_lists; ++q) {
+                if (ids) ids[k + q] = h_ids[base + q];
+                if (lps) lps[k + q] = h_lp[base + q];
+            }
+            k += r.cnt;
+        }
+        f0 += Tn;
+        if (is_prob) is_prob[u] = isp[u];
+    }
+    *n_entries = static_cast<int64_t>(k);
     return 0;
 }
 

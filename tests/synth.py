@@ -20,6 +20,7 @@ Regimes: "peaky" (margin 8, conf 0.10) is the headline, "diffuse" (margin 6, con
 stress case.
 """
 import hashlib
+import math
 import os
 import tempfile
 
@@ -235,7 +236,12 @@ class CharWorkload:
     """Vocab A or B with optional synthetic n-gram model."""
 
     def __init__(self, vocab="B", n_words=20000, lm_order=0, seed=1):
-        if vocab == "A":
+        if isinstance(vocab, int):             # a generic alphabet of `vocab` normalised labels (stream_labels)
+            self.labels = stream_labels(vocab)[:-1]
+            self.norm_labels = self.labels + [""]
+            letters = self.labels[1:]
+            self.space_id, self.blank_id = 0, len(self.labels)
+        elif vocab == "A":
             self.labels = list(LIBRI_LABELS)
             self.norm_labels = self.labels + [""]
             letters = self.labels[1:]
@@ -300,8 +306,9 @@ class BpeWorkload:
                 for i in range(1, len(w) - L + 1):
                     cont_cnt[w[i:i + L]] = cont_cnt.get(w[i:i + L], 0.0) + p
         n_special = 2  # <unk>, <pad>
-        n_start = 400 - 26
-        n_cont = V - n_special - 400 - 26
+        n_extra = V - n_special - 2 * 26             # pieces beyond the single letters in both forms
+        n_start = 400 - 26 if n_extra >= 400 - 26 else n_extra // 2
+        n_cont = n_extra - n_start
         starts = [s for s, _ in sorted(start_cnt.items(), key=lambda kv: (-kv[1], kv[0]))[:n_start]]
         conts = [s for s, _ in sorted(cont_cnt.items(), key=lambda kv: (-kv[1], kv[0]))[:n_cont]]
         self.labels = ["<unk>", "<pad>"] + [BPE + c for c in letters] + [BPE + s for s in starts] + letters + conts
@@ -374,3 +381,208 @@ def special_step_cases(wl, n_cases=60, seed=7):
         kw = dict(beam_width=int(rng.choice([2, 5, 17, 50, 100, 128])), prune_history=bool(i % 2),
                   beam_prune_logp=float(rng.choice([-10.0, -3.0, -20.0])), token_min_logp=float(rng.choice([-5.0, -3.0, -7.0])))
         yield x, kw
+
+
+# ---- streaming-stage (K1) inputs ---------------------------------------------------------------------------------------
+# Named cases for the token-list parity tests (tests/streaming_stage.py), shared by the hostsim and the GPU suite.  A case
+# is a cheap spec; `stream_case_arrays` builds its seeded utterances.  Every alphabet size and row layout the streaming
+# stage branches on is named here -- the route table is in tests/test_gpu_streaming_stage.py.
+STREAM_V = (1, 2, 3, 5, 8, 29, 31, 32, 33, 36, 63, 64, 65, 127, 128, 129, 1023, 1024, 1025, 4097)
+STREAM_T = (33, 0, 1, 7, 8, 9, 31, 32, 257)        # ragged; a non-empty first utterance keeps device batches in place
+STREAM_LOG_CLIP = math.log(1e-15)
+# thresholds: the default, none selected, only exact zeros, the clip value and the doubles on either side, all selected
+STREAM_THR = {"m5": -5.0, "p05": 0.5, "zero": 0.0, "clip": STREAM_LOG_CLIP, "clip_lo": math.nextafter(STREAM_LOG_CLIP, -math.inf),
+              "clip_hi": math.nextafter(STREAM_LOG_CLIP, math.inf), "m40": -40.0, "ninf": -math.inf}
+# pairs of columns that share the row maximum; at V == 32 they sit in different quads of the rotated LDS.128 walk
+STREAM_TIES = ((4, 28), (0, 16), (8, 12), (2, 3), (1, 30), (20, 24), (0, 31))
+
+
+def stream_labels(V):
+    """A character alphabet of exactly V normalised labels: space, V - 2 letters, blank (V = 1: blank only)."""
+    if V == 1:
+        return [""]
+    chars = [chr(0x61 + i) if i < 26 else chr(0x4E00 + i) for i in range(V - 2)]
+    return [" "] + chars + [""]
+
+
+def _row(rng, kind, V, t):
+    x = rng.standard_normal(V)
+    if kind == "peaky":
+        x[rng.integers(V)] += 8.0
+    elif kind == "flat":                       # a V-way tie
+        x[:] = 0.0
+    elif kind == "int":
+        x = np.round(x * 3.0)
+    elif kind == "tie":                        # two columns share the maximum: the lower index is the arg-max
+        i, j = STREAM_TIES[t % len(STREAM_TIES)]
+        i, j = i % V, j % V
+        x[i] = x[j] = x.max() + 4.0
+    elif kind == "nsel":                       # exactly k tokens at log-prob ~ -log k, the rest far below any threshold
+        k = (1, 3, 4, V)[t % 4]
+        x[:] = -30.0
+        x[rng.choice(V, size=min(k, V), replace=False)] = 0.0
+    elif kind == "masked":                     # -inf entries (masked vocabulary), never the best token
+        tgt = rng.integers(V)
+        x[tgt] += 8.0
+        m = rng.random(V) < 0.3
+        m[tgt] = False
+        x[m] = -np.inf
+    elif kind == "tiny":
+        x *= 1e-30
+    elif kind == "big":
+        x *= 1e4
+    elif kind == "nan0":
+        x[0] = np.nan
+    elif kind == "nan":
+        x[rng.integers(V)] = np.nan
+    elif kind == "posinf":
+        x[rng.integers(V)] = np.inf
+    elif kind == "neginf":                     # an all -inf row
+        x[:] = -np.inf
+    elif kind == "huge":                       # finite, but sum |x| overflows float32 and x - max overflows to -inf
+        x[0] = 3e38
+        if V > 1:
+            x[1 + rng.integers(V - 1)] = -3e38
+    elif kind == "huge2":                      # the same split over two lanes of a warp: each lane's partial sum is finite
+        x[0] = 2e38
+        if V > 1:
+            x[1] = -2e38
+    return x
+
+
+STREAM_FINITE_KINDS = ("peaky", "flat", "int", "tie", "nsel", "masked", "tiny", "big")
+STREAM_SPECIAL_KINDS = ("nan0", "peaky", "nan", "posinf", "neginf", "huge", "huge2", "int")
+
+
+def _to_bf16_values(x):
+    """float32 array -> the nearest bfloat16 values (round to nearest even), still stored as float32."""
+    b = np.ascontiguousarray(x, dtype=np.float32).view(np.uint32)
+    r = ((b.astype(np.uint64) + 0x7FFF + ((b >> 16) & 1)) & 0xFFFF0000).astype(np.uint32)
+    r = np.where(np.isnan(x), b, r)
+    return r.view(np.float32)
+
+
+def _prob_utterances(rng, content, V, dtype):
+    """Probabilities-or-logits inputs: (list of [T, V] float64 matrices, dtype)."""
+    out = []
+    for i, T in enumerate(STREAM_T):
+        x = rng.standard_normal((T, V)) * 2.0
+        if content == "softmax" or (content == "mixed_prob" and i % 2 == 0):
+            e = np.exp(x - x.max(1, keepdims=True)) if T else x
+            x = (e / e.sum(1, keepdims=True)) if T else x
+            x = x.astype(dtype)
+        elif content == "onehot":              # integer rows that sum to exactly 1
+            x = np.zeros((T, V))
+            x[np.arange(T), rng.integers(0, V, T)] = 1.0
+            x = x.astype(dtype)
+        elif content in ("isclose_in", "isclose_out"):
+            x = _isclose_rows(rng, T, V, dtype, content == "isclose_in")
+        elif content == "cancel":              # +-1e4 pairs that cancel, plus one 1: a row sum of about 1 after heavy cancellation
+            x = np.zeros((T, V))
+            for t in range(T):
+                cols = rng.permutation(V)
+                for a, b in zip(cols[0::2], cols[1::2]):
+                    v = rng.uniform(1e4, 2e4)
+                    x[t, a], x[t, b] = v, -v
+                x[t, cols[-1]] += 1.0
+            x = x.astype(dtype)
+        else:
+            x = x.astype(dtype)
+        out.append(x)
+    return out
+
+
+def _isclose_rows(rng, T, V, dtype, inside):
+    """Logit-looking rows whose numpy mean row sum lands just inside / just outside math.isclose(., 1)."""
+    if T == 0:
+        return np.zeros((0, V), dtype)
+    if dtype == np.float32:
+        # integers summing to exactly 1 per row (every partial sum exact in float32); outside: 2^-8 more on every row
+        x = np.round(rng.standard_normal((T, V)) * 3.0)
+        x[:, 0] += 1.0 - x.sum(1)
+        if not inside:
+            x[:, 0] += 2.0 ** -8
+        x = x.astype(np.float32)
+    else:
+        target = 1.0 + (5e-10 if inside else 3e-9)
+        x = rng.standard_normal((T, V))
+        x[:, 0] += target - x.sum(1)
+    mean = float(x.sum(axis=1).mean())
+    assert math.isclose(mean, 1) == inside, (mean, inside)
+    return x
+
+
+def streaming_stage_cases(device_routes=True):
+    """(name, V, content, dtype, route, thr) specs.  Routes: host_list (list of host arrays), host_block (one [B, T, V]
+    float32 host block called twice: the second call is pipelined), dev_inplace (adjacent slices of one device tensor),
+    dev_offset1 (the same, storage offset one element: rows not 16-byte aligned), dev_gather (separately placed device
+    tensors, more than four: the gather kernel).  Contents: mixed (finite rows of every kind), special (NaN / inf /
+    overflow rows), the probability inputs of _prob_utterances; thr is a key of STREAM_THR or ("lp", side): the float32
+    log-prob of a chosen token ("at") or the next double above it ("above")."""
+    cases = []
+
+    def add(content, V, dtype, route, thr):
+        name = "%s-V%d-%s-%s-%s" % (content, V, dtype, route, thr if isinstance(thr, str) else "lp_" + thr[1])
+        cases.append((name, V, content, dtype, route, thr))
+
+    for V in STREAM_V:
+        add("mixed", V, "f32", "host_list", "m5")
+        add("mixed", V, "f32", "host_list", "p05")
+        add("special", V, "f32", "host_list", "m5")
+    for V in (3, 29, 32, 36, 64, 65, 1024, 1025):
+        for thr in ("zero", "clip", "clip_lo", "clip_hi", "m40", "ninf"):
+            add("mixed", V, "f32", "host_list", thr)
+    for V in (5, 32, 36, 64, 65, 1024, 1025):
+        add("mixed", V, "f32", "host_list", ("lp", "at"))
+        add("mixed", V, "f32", "host_list", ("lp", "above"))
+    for V in (2, 5, 32, 33, 64, 65, 1024, 1025):
+        add("mixed", V, "f64", "host_list", "m5")
+        add("special", V, "f64", "host_list", "m5")
+        add("mixed", V, "f16", "host_list", "m5")
+        add("mixed", V, "bf16", "host_list", "m5")
+    for V in (29, 32, 36, 1024, 1025):
+        add("mixed", V, "f32", "host_block", "m5")
+    add("special", 32, "f32", "host_block", "m5")
+    for V in (5, 32, 36, 1024):
+        for content in ("softmax", "onehot", "isclose_in", "isclose_out", "cancel", "mixed_prob"):
+            add(content, V, "f32", "host_list", "m5")
+        for content in ("softmax", "isclose_in", "isclose_out"):
+            add(content, V, "f64", "host_list", "m5")
+    if device_routes:
+        for V in (1, 5, 31, 32, 33, 36, 64, 65, 1023, 1024, 1025, 4097):
+            add("mixed", V, "f32", "dev_inplace", "m5")
+            add("mixed", V, "f32", "dev_offset1", "m5")
+            add("special", V, "f32", "dev_offset1", "m5")
+            add("mixed", V, "f32", "dev_gather", "m5")
+            add("mixed", V, "f64", "dev_gather", "m5")
+            add("mixed", V, "f16", "dev_inplace", "m5")
+            add("mixed", V, "bf16", "dev_inplace", "m5")
+        for V in (5, 32, 36, 1024):
+            add("mixed_prob", V, "f32", "dev_inplace", "m5")
+            add("mixed_prob", V, "f64", "dev_gather", "m5")
+    return cases
+
+
+def stream_case_arrays(case):
+    """The seeded utterances of a case: a list of [T, V] numpy matrices in the case's dtype (bfloat16 cases: float32
+    matrices holding bfloat16 values).  host_block cases: three utterances of T = 257."""
+    name, V, content, dtype, route, thr = case
+    seed = int(hashlib.sha1(name.encode()).hexdigest()[:8], 16)
+    rng = np.random.default_rng(seed)
+    npdt = {"f32": np.float32, "f64": np.float64, "f16": np.float32, "bf16": np.float32}[dtype]
+    Ts = (257, 257, 257) if route == "host_block" else STREAM_T
+    if content in ("mixed", "special"):
+        kinds = STREAM_FINITE_KINDS if content == "mixed" else STREAM_SPECIAL_KINDS
+        xs = []
+        for u, T in enumerate(Ts):
+            rows = [_row(rng, kinds[(t + u) % len(kinds)], V, t) for t in range(T)]
+            with np.errstate(over="ignore", invalid="ignore"):
+                xs.append(np.array(rows, dtype=npdt).reshape(T, V))
+    else:
+        xs = _prob_utterances(rng, content, V, npdt)
+    if dtype == "f16":
+        with np.errstate(over="ignore"):
+            xs = [x.astype(np.float16) for x in xs]
+    elif dtype == "bf16":
+        xs = [_to_bf16_values(x) for x in xs]
+    return xs

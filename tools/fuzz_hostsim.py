@@ -24,6 +24,13 @@ FAMS = {
     "B_5gram": (dict(kind="char", vocab="B", n_words=150, lm_order=5), dict(alpha=0.9, beta=0.3, unk_score_offset=-4.0)),
     "C_bpe": (dict(kind="bpe", n_words=400, lm_order=0), {}),
     "C_bpe_4gram": (dict(kind="bpe", n_words=400, lm_order=4), dict(alpha=0.7, beta=2.0)),
+    "G5": (dict(kind="char", vocab=5, n_words=300, lm_order=0), {}),
+    "G36_3gram": (dict(kind="char", vocab=36, n_words=400, lm_order=3), dict(alpha=0.5, beta=1.0)),
+    "G64": (dict(kind="char", vocab=64, n_words=400, lm_order=0), {}),
+    "G65_2gram": (dict(kind="char", vocab=65, n_words=400, lm_order=2), dict()),
+    "G1025": (dict(kind="char", vocab=1025, n_words=400, lm_order=0), {}),
+    "C_bpe64": (dict(kind="bpe", n_words=400, lm_order=0, V=64), {}),
+    "C_bpe2000_3gram": (dict(kind="bpe", n_words=3000, lm_order=3, V=2000), dict(alpha=0.5, beta=1.0)),
 }
 
 
