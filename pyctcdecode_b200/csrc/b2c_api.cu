@@ -47,6 +47,7 @@ static int fail(int code, const std::string& msg) {
         if (_e != cudaSuccess)                                                                \
             return fail(B2C_E_CUDA, std::string(#expr) + ": " + cudaGetErrorString(_e));     \
     } while (0)
+#define B2C_TRY(expr) do { const int _rc = (expr); if (_rc) return _rc; } while (0)   // pass a stage's error on
 
 // =========================================================================================
 // workspace layout (shared memory + per-slot HBM workspace), computed on the host and
@@ -410,44 +411,42 @@ __global__ void __launch_bounds__(kThreads, kOcc) b2c_beam_kernel(const B2cBeamA
 // =========================================================================================
 // objects
 // =========================================================================================
-struct DevBuf {
+// streams, events and growing device / pinned buffers, released by their owner (the decoder)
+template <class H, cudaError_t (*Destroy)(H)>
+struct Owned {
+    H h = nullptr;
+    Owned() = default;
+    Owned(const Owned&) = delete; Owned& operator=(const Owned&) = delete;
+    ~Owned() { if (h) Destroy(h); }
+    operator H() const { return h; }
+};
+typedef Owned<cudaStream_t, cudaStreamDestroy> Stream;
+typedef Owned<cudaEvent_t, cudaEventDestroy> Event;
+template <bool kPinned>
+struct Buf {
     void* p = nullptr;
     size_t cap = 0;
+    Buf() = default;
+    Buf(const Buf&) = delete; Buf& operator=(const Buf&) = delete;
+    ~Buf() { if (p) kPinned ? cudaFreeHost(p) : cudaFree(p); }
     int ensure(size_t bytes) {
         if (bytes <= cap) return 0;
-        if (p) cudaFree(p);
-        p = nullptr;
-        cap = 0;
+        if (p) kPinned ? cudaFreeHost(p) : cudaFree(p);
+        p = nullptr; cap = 0;
         size_t want = bytes + bytes / 8 + 256;
-        cudaError_t e = cudaMalloc(&p, want);
-        if (e != cudaSuccess) {
+        cudaError_t e = kPinned ? cudaMallocHost(&p, want) : cudaMalloc(&p, want);
+        if (e != cudaSuccess && !kPinned) {       // device memory: settle for the exact size
             e = cudaMalloc(&p, bytes);
             want = bytes;
         }
-        if (e != cudaSuccess) { p = nullptr; return fail(B2C_E_NOMEM, std::string("cudaMalloc: ") + cudaGetErrorString(e)); }
+        if (e != cudaSuccess) { p = nullptr; return fail(B2C_E_NOMEM, std::string(kPinned ? "cudaMallocHost: " : "cudaMalloc: ") + cudaGetErrorString(e)); }
         cap = want;
         return 0;
     }
-    void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
     template <class U> U* as() const { return static_cast<U*>(p); }
 };
-struct PinBuf {
-    void* p = nullptr;
-    size_t cap = 0;
-    int ensure(size_t bytes) {
-        if (bytes <= cap) return 0;
-        if (p) cudaFreeHost(p);
-        p = nullptr;
-        cap = 0;
-        size_t want = bytes + bytes / 8 + 256;
-        cudaError_t e = cudaMallocHost(&p, want);
-        if (e != cudaSuccess) { p = nullptr; return fail(B2C_E_NOMEM, std::string("cudaMallocHost: ") + cudaGetErrorString(e)); }
-        cap = want;
-        return 0;
-    }
-    void release() { if (p) cudaFreeHost(p); p = nullptr; cap = 0; }
-    template <class U> U* as() const { return static_cast<U*>(p); }
-};
+typedef Buf<false> DevBuf;
+typedef Buf<true> PinBuf;
 
 struct b2c_lm {
     B2cLmHost host;
@@ -533,7 +532,7 @@ struct HostPool {
 struct b2c_decoder {
     std::unique_ptr<HostPool> pool;
     int device = 0;
-    cudaStream_t stream = nullptr;
+    Stream stream;
     int V = 0, is_bpe = 0, has_dup_labels = 0;
     std::vector<std::string> labels, clean;
     std::vector<B2cTok> toks;
@@ -548,18 +547,18 @@ struct b2c_decoder {
     DevBuf d_raw, d_lmx, d_stream, d_mstats, d_sumk, d_clk, d_maxk, d_toks, d_logits, d_meta, d_tok_start, d_tok_ids, d_tok_lp, d_rowsum, d_set, d_isprob, d_approx, d_ws, d_hot, d_states,
         d_out_small, d_out_toks, d_out_frames;
     PinBuf h_sumk, h_maxk, h_meta, h_out_small, h_out_toks, h_out_frames, h_mstats;
-    cudaEvent_t ev[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
-    cudaStream_t cls_stream[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};   // one per capacity class
-    cudaEvent_t cls_done[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
-    cudaEvent_t fork_ev = nullptr;
-    cudaEvent_t caller_ev = nullptr;      // b2c_decoder_wait_stream: the caller's stream at the time of the call
+    Event ev[6];
+    Stream cls_stream[2];                 // concurrent launches of a call: the fast class, the general kernel
+    Event cls_done[2];
+    Event fork_ev;
+    Event caller_ev;                      // b2c_decoder_wait_stream: the caller's stream at the time of the call
     // pipelined calls (host input): chunks along T are copied on copy_stream while earlier chunks are decoded
-    cudaStream_t copy_stream = nullptr;
-    cudaEvent_t copied[B2C_PIPE_CHUNKS] = {nullptr, nullptr, nullptr, nullptr};
-    cudaEvent_t chunk_ev[3 * B2C_PIPE_CHUNKS] = {};
+    Stream copy_stream;
+    Event copied[B2C_PIPE_CHUNKS];
+    Event chunk_ev[3 * B2C_PIPE_CHUNKS];
     DevBuf d_state, d_gate;
-    cudaStream_t prep_stream = nullptr;   // gated pipelined calls: streaming stage of the later chunks, concurrent with the beam kernel
-    cudaEvent_t prep_ev[3] = {nullptr, nullptr, nullptr};    // inputs ready / first chunk streamed / all streamed and decided
+    Stream prep_stream;                   // gated pipelined calls: streaming stage of the later chunks, concurrent with the beam kernel
+    Event prep_ev[3];                     // inputs ready / first chunk streamed / all streamed and decided
     bool pipe_refused = false;            // the last pipelined attempt of this configuration could not be planned
     double last_device_ms = 0.0;          // streaming stage + beam kernel of the previous call (chunk sizing of pipelined calls)
     int plain_v5 = -2, plain_cap = 0;     // kernel variant / capacity class of the last PLAIN call (pipelined calls must plan the same)
@@ -706,55 +705,240 @@ static void assemble_beam(const b2c_decoder* d, const u32* toks, int nt, const i
     br.frames.resize(n * 2);
 }
 
-struct MetaHost {   // one pinned staging block -> one H2D copy
-    std::vector<u64> frame_off;
-    std::vector<int> T, order;
+// =========================================================================================
+// one decode call: its shape, switches, buffer layouts and launch plan
+// =========================================================================================
+// capacity classes of the shared-memory candidate tier
+static const int kNumCaps = 6;
+static const u32 kCaps[kNumCaps] = {128, 256, 512, 1024, 2048, 4096};
+// big classes leave room for one CTA per SM only: give that CTA 256 threads (a diffuse frame has ~650 candidates)
+static int threads_of(int c) { return kCaps[c] <= 128 ? 32 : (kCaps[c] <= 256 ? 64 : (kCaps[c] >= 2048 ? 256 : 128)); }
+static int per_sm_of(u32 smem_bytes, int threads) {
+    const int by_smem = static_cast<int>(std::max<u64>(1, (224 * 1024) / std::max<u32>(smem_bytes + 1024, 2048)));
+    return std::min(by_smem, threads == 32 ? 8 : (threads == 64 ? 4 : (threads >= 256 ? 1 : 2)));
+}
+
+// one beam launch: utterances [ord_off, ord_off + count) of the work list, capacity class cls (kNumCaps: general kernel),
+// v5 >= 0: variant of the latency-first kernel (b2c_beam_fast.h; L.smem_bytes is kV5Smem[v5] then)
+struct Launch { int cls; size_t ord_off; int count; B2cLayout L; int slots; int per_sm; int threads; int v5; };
+// the shape of a call: what its launch plan is made from besides the token statistics and the decoder's hint
+struct Geometry {
+    int n_utts = 0, V = 0, beam_width = 0, W_tab = 0, n_lm = 1, s_max_beams = 0, T_max = 0;
+    u64 s_max_words = 0, total_frames = 0;
+    size_t esz = 4;               // element size of the logits the streaming stage reads
+    bool streaming = false, hint_ok = false, pipelined = false;
+    u32 smem_budget = 0;
+    const int32_t* T = nullptr;
+    const int* order = nullptr;   // utterance ids, longest first
+};
+// the B200CTC_* switches (INTEGRATION.md §3), read at every call so that tests can change them between calls
+struct Knobs {
+    bool host_prof, no_pipe, no_hinted, force_v5, no_v5, no_lean, force_lean, pipe_all, no_gate, gate_early;
+    int v5_variant, force_chunks;  // v5_variant -1: chosen from the hint
+};
+static bool env_set(const char* name) { return std::getenv(name) != nullptr; }
+static Knobs read_knobs() {
+    Knobs k;
+    k.host_prof = env_set("B200CTC_HOST_PROFILE");        // host-side section timing on stderr
+    k.no_pipe = env_set("B200CTC_NO_PIPELINE") || !env_switch("B200CTC_PIPELINE", B2C_DEFAULT_PIPELINE != 0);
+    k.no_hinted = env_set("B200CTC_NO_HINTED");
+    k.force_v5 = env_set("B200CTC_FORCE_V5");             // tests: exercise the out-of-line step
+    k.no_v5 = env_set("B200CTC_NO_V5");
+    const char* v = std::getenv("B200CTC_V5_VARIANT"), *fc = std::getenv("B200CTC_FORCE_CHUNKS");
+    k.v5_variant = v ? std::max(0, std::min(2, std::atoi(v))) : -1;
+    k.no_lean = env_set("B200CTC_NO_LEAN") || !env_switch("B200CTC_LEAN", B2C_DEFAULT_LEAN != 0);
+    k.force_lean = env_set("B200CTC_FORCE_LEAN");
+    k.force_chunks = fc ? std::atoi(fc) : 0;              // tests
+    k.pipe_all = env_set("B200CTC_PIPELINE_ALL"); k.no_gate = env_set("B200CTC_NO_GATE");
+    k.gate_early = env_set("B200CTC_HOSTSIM_GATE_EARLY");  // hostsim tests: the later chunks of a gated launch never arrive
+    return k;
+}
+struct Plan {
+    std::vector<Launch> launches;
+    std::vector<int> ord;         // the work list: utterances of the launches, launch by launch
+    bool use_v5 = false, use_lean = false;
+    int v5_variant = 0;
+    std::vector<int> bounds;      // chunk boundaries along T ({0, T_max}: one chunk)
+    bool gated = false;           // chunks feed ONE beam launch through device flags
+    bool redo_plain = false;      // a pipelined call that cannot be planned as one: redo it as a plain call
 };
 
-// streaming pass (every utterance as logits) -> decide (exact only where the approximate mean row sum is near 1) ->
-// second pass over the utterances that turned out to be probabilities (returns at once when there is none)
-template <class T>
-static int launch_prepare(b2c_decoder* d, const B2cPrepArgs& A0, int n_utts, int grid_tile, int grid_tok) {
-    B2cPrepArgs A = A0, A1 = A0;
-    A.mode = 0;
-    A1.mode = 1;
+// the metadata block, pinned on the host and mirrored on the device: [n] frame offsets (at 0), [n] T, [n + 1] run offsets
+// (these three go up in one copy), [2n] work list (class lists, then the retry list), [16] queue heads (one per launch),
+// [n] source pointers of a gather launch
+struct MetaLayout {
+    size_t T, run, ord, next, ptr, bytes;
+    explicit MetaLayout(int n = 0)
+        : T(al16(8ull * n)), run(T + al16(4ull * n)), ord(run + al16(8ull * (n + 1))), next(ord + 2 * al16(4ull * n)), ptr(next + 64),
+          bytes(ptr + al16(8ull * n)) {}
+};
+// the small-output block (device, then pinned host copy)
+struct OutViews {
+    int *nbeams, *status; double* scores; int *ntok, *nwords; B2cLmState* states;
+    int* aux;                     // streaming calls only
+    B2cLmState* states_x;         // MultiLanguageModel only
+};
+struct OutLayout {
+    u64 st = 0, sc = 0, nt = 0, nw = 0, ls = 0, ax = 0, lx = 0, bytes = 0;   // n_beams at 0
+    bool has_aux = false, has_x = false;
+    OutLayout() = default;
+    OutLayout(int n, int OB, int n_lm, bool streaming)
+        : st(al16(4ull * n)), sc(st + al16(4ull * n)), nt(sc + al16(16ull * OB * n)), nw(nt + al16(4ull * OB * n)), ls(nw + al16(4ull * OB * n)),
+          ax(ls + al16(sizeof(B2cLmState) * static_cast<u64>(OB) * n)), lx(ax + (streaming ? al16(16ull * OB * n) : 0)),
+          bytes(lx + al16(sizeof(B2cLmState) * static_cast<u64>(OB) * n * static_cast<u64>(n_lm - 1))), has_aux(streaming), has_x(n_lm > 1) {}
+    OutViews at(u8* b) const {
+        return OutViews{reinterpret_cast<int*>(b), reinterpret_cast<int*>(b + st), reinterpret_cast<double*>(b + sc),
+                        reinterpret_cast<int*>(b + nt), reinterpret_cast<int*>(b + nw), reinterpret_cast<B2cLmState*>(b + ls),
+                        has_aux ? reinterpret_cast<int*>(b + ax) : nullptr, has_x ? reinterpret_cast<B2cLmState*>(b + lx) : nullptr};
+    }
+};
+
+// opt-in host-side section timing (B200CTC_HOST_PROFILE=1, stderr)
+struct HostProfile {
+    std::chrono::steady_clock::time_point t0 = std::chrono::steady_clock::now();
+    double ms[6] = {0, 0, 0, 0, 0, 0};
+    void mark(int k) { const auto now = std::chrono::steady_clock::now(); ms[k] += std::chrono::duration<double, std::milli>(now - t0).count(); t0 = now; }
+};
+
+struct Call {
+    const void* const* logits; const int32_t* T; const b2c_decode_opts_t* opts;
+    int dtype_in;                 // B2C_DTYPE_* of the caller's matrices; half precision is widened to float32 on the device
+    bool half_in, f64, is_device, allow_pipe;
+    size_t esz_in;                // element size of the caller's matrices
+    Knobs k;
+    HostProfile hp;
+    Geometry g;
+    std::vector<u64> frame_off;
+    std::vector<int> order;
+    int OB = 1;
+    bool text_only = false;       // no word lists, no frames
+    std::vector<B2cStreamUtt> s_utts; std::vector<B2cStreamBeam> s_beams; std::vector<u64> s_wh; std::vector<u32> s_wl;
+    B2cParams P;
+    std::vector<B2cHot> hot;
+    bool contiguous_dev = false;  // device input, every utterance right behind the previous one
+    MetaLayout meta;
+    OutLayout out;
+    u64 tok_bytes = 0, frm_bytes = 0;
+    u32 set_cap = 16;
+    int runs_per_utt = 1, tiles_per_utt = 1;
+    u8 *hm = nullptr, *dm = nullptr;   // metadata block: host, device
+    const void* d_logits = nullptr;
+    B2cPrepArgs PA;
+    B2cBeamArgs BA;
+    bool hinted = false;          // planned from the hint, beam kernel enqueued right behind the streaming stage
+    std::vector<u32> nostat_maxk, nostat_sumk;
+    const u32* maxk = nullptr;    // the per-utterance token maxima the plan was made from
+    Plan plan;
+    std::vector<u64> ws_off;
+    bool chunk_timing = false, gated_call = false;
+
+    Call(const b2c_decoder* d, const void* const* lg, const int32_t* t, int n, int dtype, int dev, const b2c_decode_opts_t* o, bool pipe)
+        : logits(lg), T(t), opts(o), dtype_in(dtype), half_in(dtype == B2C_DTYPE_F16 || dtype == B2C_DTYPE_BF16), f64(dtype == B2C_DTYPE_F64),
+          is_device(dev != 0), allow_pipe(pipe), esz_in(half_in ? 2 : (f64 ? 8 : 4)), k(read_knobs()) {
+        g.n_utts = n; g.V = d->V; g.beam_width = o->beam_width; g.esz = f64 ? 8 : 4; g.T = t;
+        std::memset(&P, 0, sizeof(P)); std::memset(&PA, 0, sizeof(PA)); std::memset(&BA, 0, sizeof(BA));
+    }
+    int* h_ord() const { return reinterpret_cast<int*>(hm + meta.ord); }
+    int* d_ord() const { return reinterpret_cast<int*>(dm + meta.ord); }
+    u32* d_next() const { return reinterpret_cast<u32*>(dm + meta.next); }
+};
+
+// =========================================================================================
+// launch helpers: the only places where the CUDA build and hostsim differ
+// =========================================================================================
+static int grid_of(const b2c_decoder* d, u64 items, int per_block) {
+    return static_cast<int>(std::max<u64>(1, std::min<u64>((items + per_block - 1) / per_block, static_cast<u64>(d->n_sm) * 8)));
+}
+
+// one pass of the streaming stage over tiles [tile_lo, tile_hi) / runs [run_lo, run_hi) of every utterance: the
+// lane-per-row tile kernel (float32, V <= 32, streaming pass) or the warp kernel
+static int launch_tokens(b2c_decoder* d, const B2cPrepArgs& A, bool f64, cudaStream_t s) {
+    const int grid = grid_of(d, static_cast<u64>(A.n_utts) * static_cast<u64>(A.run_hi - A.run_lo), B2C_PREP_WARPS);
+    d->tm.launches += 1;
 #ifdef B2C_HOSTSIM
-    (void)d;
-    (void)grid_tile;
     std::unique_ptr<B2cPrepShared> sh(new B2cPrepShared());
-    for (int b = 0; b < grid_tok; ++b) b2c_tokens_block<T>(A, b, grid_tok, sh.get());
-    std::unique_ptr<B2cDecideShared> dsh(new B2cDecideShared());
-    for (int u = 0; u < n_utts; ++u) b2c_decide_block<T>(A, u, dsh.get());
-    for (int b = 0; b < grid_tok; ++b) b2c_tokens_block<T>(A1, b, grid_tok, sh.get());
+    for (int b = 0; b < grid; ++b) {
+        if (f64) b2c_tokens_block<double>(A, b, grid, sh.get());
+        else b2c_tokens_block<float>(A, b, grid, sh.get());
+    }
 #else
-    if (sizeof(T) == 4 && A.V <= 32) b2c_tokens_tile_kernel<<<grid_tile, B2C_TILE_WARPS * 32, 0, d->stream>>>(A);
-    else b2c_tokens_kernel<T><<<grid_tok, B2C_PREP_THREADS, 0, d->stream>>>(A);
-    b2c_decide_kernel<T><<<n_utts, 128, 0, d->stream>>>(A);
-    b2c_tokens_kernel<T><<<grid_tok, B2C_PREP_THREADS, 0, d->stream>>>(A1);
+    if (!f64 && A.mode == 0 && A.V <= 32)
+        b2c_tokens_tile_kernel<<<grid_of(d, static_cast<u64>(A.n_utts) * static_cast<u64>(A.tile_hi - A.tile_lo), B2C_TILE_WARPS),
+                                 B2C_TILE_WARPS * 32, 0, s>>>(A);
+    else if (f64) b2c_tokens_kernel<double><<<grid, B2C_PREP_THREADS, 0, s>>>(A);
+    else b2c_tokens_kernel<float><<<grid, B2C_PREP_THREADS, 0, s>>>(A);
     CUDA_OK(cudaGetLastError());
 #endif
     return 0;
 }
 
-// v5 >= 0: variant of the latency-first kernel (b2c_beam_fast.h); A.L.smem_bytes is kV5Smem[v5] then
-static int launch_beam(b2c_decoder* d, const B2cBeamArgs& A, int slots, bool fast, int per_sm, int threads, cudaStream_t stream,
-                       int v5 = -1) {
+// probabilities or logits, per utterance (exact only where the approximate mean row sum is near 1)
+static int launch_decide(b2c_decoder* d, const B2cPrepArgs& A, bool f64, cudaStream_t s) {
+    d->tm.launches += 1;
 #ifdef B2C_HOSTSIM
-    (void)d;
+    std::unique_ptr<B2cDecideShared> sh(new B2cDecideShared());
+    for (int u = 0; u < A.n_utts; ++u) {
+        if (f64) b2c_decide_block<double>(A, u, sh.get());
+        else b2c_decide_block<float>(A, u, sh.get());
+    }
+#else
+    if (f64) b2c_decide_kernel<double><<<A.n_utts, 128, 0, s>>>(A);
+    else b2c_decide_kernel<float><<<A.n_utts, 128, 0, s>>>(A);
+    CUDA_OK(cudaGetLastError());
+#endif
+    return 0;
+}
+
+static int launch_widen(b2c_decoder* d, const u16* src, float* dst, u64 n, int bf16, cudaStream_t s) {
+    d->tm.launches += 1;
+#ifdef B2C_HOSTSIM
+    b2c_widen_range(src, dst, 0, n, 1, bf16);
+#else
+    const int blocks = static_cast<int>(std::min<u64>((n + 255) / 256, static_cast<u64>(d->n_sm) * 16));
+    b2c_widen_kernel<<<blocks, 256, 0, s>>>(src, dst, n, bf16);
+    CUDA_OK(cudaGetLastError());
+#endif
+    return 0;
+}
+
+#define B2C_NO_GATHER 1   // launch_gather: this build has no gather kernel (hostsim), the caller copies the utterances
+static int launch_gather(b2c_decoder* d, const Call& c) {
+#ifdef B2C_HOSTSIM
+    (void)d; (void)c;
+    return B2C_NO_GATHER;
+#else
+    const int n = c.g.n_utts;
+    const void** h_ptr = reinterpret_cast<const void**>(c.hm + c.meta.ptr);
+    for (int i = 0; i < n; ++i) h_ptr[i] = c.logits[i];
+    CUDA_OK(cudaMemcpyAsync(c.dm + c.meta.ptr, h_ptr, 8ull * n, cudaMemcpyHostToDevice, d->stream));
+    const int chunks = std::max(1, std::min(64, (d->n_sm * 8 + n - 1) / n));
+    b2c_gather_kernel<<<n * chunks, 256, 0, d->stream>>>(reinterpret_cast<const void* const*>(c.dm + c.meta.ptr),
+                                                         reinterpret_cast<const u64*>(c.dm), reinterpret_cast<const int*>(c.dm + c.meta.T),
+                                                         static_cast<u64>(c.g.V) * (c.g.esz / 4), d->d_logits.as<u32>(), n, chunks);
+    CUDA_OK(cudaGetLastError());
+    d->tm.launches += 1;
+    return 0;
+#endif
+}
+
+// one beam launch; `record`: its shape goes into the timings (cap_candidates, cta_threads, cta_slots, kernel_variant)
+static int launch_beam(b2c_decoder* d, const B2cBeamArgs& A, const Launch& ln, cudaStream_t stream, bool record) {
+    const int slots = ln.slots, v5 = ln.v5, threads = ln.threads;
+    const bool fast = ln.cls < kNumCaps;
+    d->tm.launches += 1;
+    if (record) {
+        d->tm.cap_candidates = static_cast<int>(ln.L.cap_s); d->tm.cta_threads = threads; d->tm.cta_slots = slots;
+        d->tm.kernel_variant = v5 >= 0 ? 2 : (fast ? 1 : 0);
+    }
+#ifdef B2C_HOSTSIM
     (void)stream;
-    (void)per_sm;
-    (void)threads;
     std::vector<u8> smem(A.L.smem_bytes + 64);
     const bool table = A.P.V <= B2C_FAST_LT;
     for (int s = 0; s < slots; ++s) {
-        if (v5 == 0 && table) b2c_beam_block_fast<128, 1024, B2C_FAST_LT>(A, s, smem.data());
-        else if (v5 == 0) b2c_beam_block_fast<128, 1024, 0>(A, s, smem.data());
-        else if (v5 == 1 && table) b2c_beam_block_fast<128, 512, B2C_FAST_LT>(A, s, smem.data());
-        else if (v5 == 1) b2c_beam_block_fast<128, 512, 0>(A, s, smem.data());
-        else if (v5 == 2 && table) b2c_beam_block_fast<128, 256, B2C_FAST_LT>(A, s, smem.data());
-        else if (v5 == 2) b2c_beam_block_fast<128, 256, 0>(A, s, smem.data());
-        else if (v5 == 3 && table) b2c_beam_block_fast<32, 128, B2C_FAST_LT>(A, s, smem.data());
-        else if (v5 == 3) b2c_beam_block_fast<32, 128, 0>(A, s, smem.data());
+        if (v5 == 0) table ? b2c_beam_block_fast<128, 1024, B2C_FAST_LT>(A, s, smem.data()) : b2c_beam_block_fast<128, 1024, 0>(A, s, smem.data());
+        else if (v5 == 1) table ? b2c_beam_block_fast<128, 512, B2C_FAST_LT>(A, s, smem.data()) : b2c_beam_block_fast<128, 512, 0>(A, s, smem.data());
+        else if (v5 == 2) table ? b2c_beam_block_fast<128, 256, B2C_FAST_LT>(A, s, smem.data()) : b2c_beam_block_fast<128, 256, 0>(A, s, smem.data());
+        else if (v5 == 3) table ? b2c_beam_block_fast<32, 128, B2C_FAST_LT>(A, s, smem.data()) : b2c_beam_block_fast<32, 128, 0>(A, s, smem.data());
         else if (fast) b2c_beam_block<true>(A, s, smem.data());
         else b2c_beam_block<false>(A, s, smem.data());
     }
@@ -785,7 +969,6 @@ static int launch_beam(b2c_decoder* d, const B2cBeamArgs& A, int slots, bool fas
             CUDA_OK(cudaFuncSetAttribute(b2c_beam_kernel<FAST, THREADS, OCC>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)); \
         b2c_beam_kernel<FAST, THREADS, OCC><<<slots, THREADS, A.L.smem_bytes, stream>>>(A);                           \
     } while (0)
-    (void)per_sm;
     if (fast && threads == 32) B2C_LAUNCH_BEAM(true, 32, 8);           // 255 registers x 32 threads: 8 one-warp CTAs per SM
     else if (fast && threads == 256) B2C_LAUNCH_BEAM(true, 256, 1);    // 255 registers x 256 threads: the whole register file
     else if (fast && threads == 64) B2C_LAUNCH_BEAM(true, 64, 4);     // 255 registers x 64 threads: 4 CTAs per SM
@@ -797,6 +980,191 @@ static int launch_beam(b2c_decoder* d, const B2cBeamArgs& A, int slots, bool fas
     CUDA_OK(cudaGetLastError());
 #endif
     return 0;
+}
+
+// =========================================================================================
+// launch plan: a function of the call's geometry, token statistics, switches and the decoder's hint, SM count and
+// shared-memory limit; it makes no CUDA call and changes nothing in the decoder
+// =========================================================================================
+static B2cLayout class_layout(const Geometry& g, int c, int tmax, bool full, u64 worst_m) {
+    // the 2048 / 4096-candidate classes own an SM anyway: they rank over the wide bucket array
+    return make_layout(g.beam_width, g.V, tmax, full, g.smem_budget, kCaps[c], worst_m, threads_of(c) / 32, 0, 0, 1,
+                       kCaps[c] >= 2048 ? B2C_NBUCKET_WIDE : B2C_NBUCKET);
+}
+static B2cLayout general_layout(const Geometry& g, int tmax, bool full, u64 worst_m, u32 cap_max) {
+    return make_layout(g.W_tab, g.V, tmax, full, g.smem_budget, 0, worst_m, B2C_MAXWARPS, static_cast<u64>(g.s_max_beams),
+                       g.s_max_words + static_cast<u64>(g.s_max_beams), g.n_lm, B2C_NBUCKET_WIDE, cap_max);
+}
+
+// the launch over `utts` in class cls (kNumCaps: the general kernel); full: worst-case arenas
+static Launch plan_launch(const Geometry& g, const u32* maxk, const Plan& p, int n_sm, const std::vector<int>& utts, int cls, bool full,
+                          size_t ord_off) {
+    Launch ln;
+    ln.cls = cls; ln.ord_off = ord_off; ln.count = static_cast<int>(utts.size());
+    int tmax = 1;
+    u32 kmax = 1;
+    for (int u : utts) {
+        tmax = std::max(tmax, static_cast<int>(g.T[u]));
+        kmax = std::max(kmax, maxk[u]);
+    }
+    const u64 worst_m = static_cast<u64>(g.W_tab) * std::min<u32>(kmax, static_cast<u32>(g.V));
+    ln.v5 = (p.use_v5 && cls < kNumCaps) ? (p.use_lean ? 3 : p.v5_variant) : -1;
+    if (ln.v5 == 3) {
+        // lean variant: 32 slots, 128 candidates, no out-of-line tier (what does not fit is handed back)
+        ln.threads = 32;
+        ln.L = make_layout(32, g.V, tmax, full, g.smem_budget, 128, 0, 1);
+        ln.L.smem_bytes = static_cast<u32>(kV5Smem[3][g.V <= B2C_FAST_LT ? 1 : 0]);
+        ln.per_sm = kV5Occ[3];
+    } else if (ln.v5 >= 0) {
+        // beam tables of capacity 128; the HBM tier always exists (frames with more tokens than the rings hold use it too)
+        const u32 cap5 = kV5Cap[ln.v5];
+        ln.threads = kV5Threads[ln.v5];
+        // backtrack arena: fixed node ids of the frame steps below 128 * T, the out-of-line step allocates above
+        ln.L = make_layout(128, g.V, tmax, full, g.smem_budget, cap5, std::max<u64>(worst_m, cap5 + 1), B2C_FAST_NW,
+                           128ull * static_cast<u64>(std::max(tmax, 1)));
+        ln.L.smem_bytes = static_cast<u32>(kV5Smem[ln.v5][g.V <= B2C_FAST_LT ? 1 : 0]);
+        ln.per_sm = kV5Occ[ln.v5];
+    } else {
+        ln.threads = cls < kNumCaps ? threads_of(cls) : 128;
+        if (cls < kNumCaps) {
+            ln.L = class_layout(g, cls, tmax, full, worst_m);
+        } else {
+            // general kernel: the largest shared-memory candidate tier that fits (frames beyond it work on the HBM tier at
+            // L2 latency) -- unless the launch has more utterances than SMs and the small tier keeps two CTAs per SM
+            ln.L = general_layout(g, tmax, full, worst_m, 2048);
+            if (per_sm_of(ln.L.smem_bytes, 128) == 1 && ln.count > n_sm) {
+                const B2cLayout small = general_layout(g, tmax, full, worst_m, 512);
+                if (per_sm_of(small.smem_bytes, 128) >= 2) ln.L = small;
+            }
+        }
+        // the general kernel with room for one CTA per SM only (wide beams): that CTA gets the whole register file --
+        // its phases are loops over hundreds to thousands of candidates, each a chain of dependent memory accesses
+        if (cls == kNumCaps && per_sm_of(ln.L.smem_bytes, 128) == 1) ln.threads = 256;
+        // beam tables that do not fit shared memory (beam_width in the thousands) live in HBM: every phase is a chain of L2
+        // round trips, and twice the threads at half the registers hide more of them (with the tables in shared memory,
+        // e.g. beam 500, the spills cost more than they hide)
+        if (cls == kNumCaps && ln.threads == 256 && !ln.L.beams_in_smem) ln.threads = 512;
+        ln.per_sm = per_sm_of(ln.L.smem_bytes, ln.threads);
+    }
+    ln.slots = std::min(ln.count, n_sm * ln.per_sm);
+    const u64 budget = 16ull << 30;            // keep the HBM workspace bounded
+    if (static_cast<u64>(ln.slots) * ln.L.gws_bytes > budget)
+        ln.slots = static_cast<int>(std::max<u64>(1, budget / ln.L.gws_bytes));
+    return ln;
+}
+
+// Chunk boundaries.  A chunked launch ends when its SLOWEST utterance has finished the chunk, so every boundary costs the
+// spread of the per-chunk times.  GATED launch (preferred for pipelined calls): ONE beam launch that starts after the
+// first chunk and waits, on the device, for the flag of each later chunk -- no launch boundary, so no chunk pays for its
+// slowest utterance.  The streaming stage of the later chunks runs CONCURRENTLY with the beam kernel on another stream,
+// which needs free SM resources: only taken when the beam kernel leaves at least n_sm/8 CTA slots empty; a CTA that
+// waits longer than ~40 ms gives up with B2C_ERR_GATE and the call is redone as a plain call.
+// Which form of pipelining:
+//   compute-bound calls (copy < 0.6 x decode, e.g. C2) -> the gated launch; without it, TWO chunks: a short first one
+//     whose decode covers the copy of the rest;
+//   copy-bound calls (e.g. the C4 shape) -> chunked launches, equal chunks (the gated form is slower there: the
+//     streaming stage of a 1 GB batch crawls on the SM slots the beam kernel leaves free).
+// The plan of a pipelined call comes from the hint alone; it must be the plan the previous plain call of this
+// configuration ran (another kernel variant would change the speed, not the result: diffuse batches decode 35 % slower
+// on the latency-first kernel the hint-only plan picks than on the capacity-class kernel their statistics pick).
+static void plan_chunks(const Geometry& g, const b2c_decoder& d, const Knobs& k, Plan& p) {
+    const int T_max = g.T_max;
+    p.bounds = {0, std::max(T_max, 0)};
+    // chunked launches need ONE launch of the latency-first kernel with every utterance resident
+    const Launch& l0 = p.launches[0];
+    const bool can_chunk = p.launches.size() == 1 && l0.v5 >= 0 && l0.count <= l0.slots && !g.streaming;
+    if (g.pipelined && !can_chunk) { p.redo_plain = true; return; }
+    const double copy_ms_est = static_cast<double>(g.total_frames) * g.V * g.esz / 50.0e6;            // ~50 GB/s pinned H2D
+    const double r = copy_ms_est / std::max(d.last_device_ms > 0 ? d.last_device_ms : copy_ms_est, 1e-3);
+    p.gated = g.pipelined && !k.no_gate && (r < 0.6 || k.pipe_all) && l0.count + d.n_sm / 8 <= d.n_sm * l0.per_sm;
+    if (g.pipelined) {
+        const bool same_plan = l0.v5 == d.plain_v5 && static_cast<int>(l0.L.cap_s) == d.plain_cap;
+        if ((!p.gated && r < 0.6 && !k.pipe_all) || (!same_plan && !k.pipe_all)) { p.redo_plain = true; return; }
+        p.bounds = {0};
+        if (!p.gated && r < 0.6) {
+            int f = static_cast<int>(1.15 * T_max * r / (1.0 + r));
+            f = std::max(2 * B2C_TILE_ROWS, ((f + B2C_TILE_ROWS - 1) / B2C_TILE_ROWS) * B2C_TILE_ROWS);
+            if (f < T_max) p.bounds.push_back(f);
+        } else {
+            const int chunk_len = ((T_max + B2C_PIPE_CHUNKS * B2C_TILE_ROWS - 1) / (B2C_PIPE_CHUNKS * B2C_TILE_ROWS)) * B2C_TILE_ROWS;
+            for (int c = 1; c < B2C_PIPE_CHUNKS; ++c) if (c * chunk_len < T_max) p.bounds.push_back(c * chunk_len);
+        }
+        p.bounds.push_back(T_max);
+    } else if (can_chunk && k.force_chunks > 1 && T_max >= 2) {
+        const int nc = std::min(k.force_chunks, T_max), cl = (T_max + nc - 1) / nc;
+        p.bounds.clear();
+        for (int t0 = 0; t0 < T_max; t0 += cl) p.bounds.push_back(t0);
+        p.bounds.push_back(T_max);
+    }
+}
+
+// maxk / sumk: per-utterance largest and total token counts -- this call's statistics, or the worst-case stand-ins of a
+// pipelined or hinted call
+static Plan make_plan(const Geometry& g, const u32* maxk, const u32* sumk, const b2c_decoder& d, const Knobs& k) {
+    Plan p;
+    // ---- capacity class of the shared-memory candidate tier (ONE fast class per call) -------------
+    // upper bound: sized for the TYPICAL frame of an utterance if all beam_width beams were alive
+    // (2.5 x its mean tokens per frame, at least 4); with a hint from the previous call of the same
+    // configuration (histogram of the per-frame candidate counts actually seen -- with an LM far fewer
+    // beams stay alive): the smallest class that covers all but 0.4% of the frames.  The few wider
+    // frames take the out-of-line HBM-tier step inside the same kernel, so every choice is exact.
+    // Small classes run 64-thread CTAs (255 registers x 64 threads: 4 CTAs per SM), the others 128.
+    bool cap_ok[kNumCaps];
+    for (int c = 0; c < kNumCaps; ++c) cap_ok[c] = class_layout(g, c, 1, false, 0).smem_bytes <= g.smem_budget;
+    std::vector<int> cls_of(g.n_utts, kNumCaps);
+    int top = -1, n_fast = 0;
+    for (int u = 0; u < g.n_utts; ++u) {
+        const double mean_k = g.T[u] > 0 ? static_cast<double>(sumk[u]) / g.T[u] : 1.0;
+        const u32 typ_k = std::min<u32>(std::max<u32>(maxk[u], 1u), std::max<u32>(4u, static_cast<u32>(std::ceil(2.5 * mean_k))));
+        const u64 need = std::min<u64>(static_cast<u64>(g.beam_width) * typ_k, static_cast<u64>(g.beam_width) * static_cast<u64>(g.V));
+        for (int c = 0; c < kNumCaps && !g.streaming && g.n_lm == 1; ++c)      // streaming / multi-LM calls take the general kernel
+            if (cap_ok[c] && need <= kCaps[c]) { cls_of[u] = c; break; }
+        if (cls_of[u] < kNumCaps) { top = std::max(top, cls_of[u]); ++n_fast; }
+    }
+    if (top >= 0 && g.hint_ok) {
+        int c_hint = kNumCaps - 1;
+        for (int c = 0; c < kNumCaps; ++c)
+            if (static_cast<double>(d.hint_over[c]) <= 0.004 * d.hint_frames) { c_hint = c; break; }
+        while (c_hint < top && !cap_ok[c_hint]) ++c_hint;
+        top = std::min(top, c_hint);
+    }
+    const int v5_top = top;                    // the class the statistics ask for, before the residency upgrade
+    // upgrade while every fast utterance stays resident (fewer frames need the out-of-line step)
+    while (top >= 0 && top + 1 < kNumCaps && cap_ok[top + 1]) {
+        const u32 sb = class_layout(g, top + 1, 1, false, 0).smem_bytes;
+        if (static_cast<long long>(d.n_sm) * per_sm_of(sb, threads_of(top + 1)) < n_fast) break;
+        ++top;
+    }
+    // beam_width <= 128 and a typical frame within 1024 candidates: the latency-first kernel (v5) takes
+    // the whole fast list; wider frames inside it go through its out-of-line HBM-tier step
+    p.use_v5 = top >= 0 && g.beam_width <= 128 && (k.force_v5 || kCaps[v5_top >= 0 ? v5_top : top] <= 1024) &&
+               kV5Smem[0][1] + 1024 <= d.smem_optin && !k.no_v5;
+    // more utterances than variant A keeps resident: trade capacity for residency if the previous call's
+    // histogram says that all but 0.4% of the frames fit (hint_over[q] = frames with > 128 << q candidates)
+    if (p.use_v5 && g.hint_ok && n_fast > d.n_sm * kV5Occ[0] && k.v5_variant < 0) {
+        for (int v = 2; v >= 1; --v) {
+            const int q = kV5Cap[v] == 256 ? 1 : 2;
+            if (static_cast<double>(d.hint_over[q]) <= 0.004 * d.hint_frames) { p.v5_variant = v; break; }
+        }
+    }
+    if (k.v5_variant >= 0) p.v5_variant = k.v5_variant;
+    // the lean one-warp variant: more utterances than the chosen variant keeps resident, and the previous call of
+    // this configuration says that (nearly) every utterance fits 32 slots / 128 candidates / 16 tokens per frame
+    p.use_lean = p.use_v5 && g.beam_width <= 128 &&
+                 (k.force_lean || (!k.no_lean && (g.hint_ok && !d.lean_bad && d.hint_utts > 0 && 20ull * d.hint_wide_utts <= d.hint_utts &&
+                                                 n_fast > d.n_sm * kV5Occ[p.v5_variant])));
+    std::vector<std::vector<int>> classes(kNumCaps + 1);   // the fast class (one per call), last = general
+    for (int q = 0; q < g.n_utts; ++q) {
+        const int u = g.order[q];             // keeps longest-first order inside every class
+        classes[cls_of[u] < kNumCaps ? top : kNumCaps].push_back(u);
+    }
+    for (int c = 0; c <= kNumCaps; ++c) {
+        if (classes[c].empty()) continue;
+        p.launches.push_back(plan_launch(g, maxk, p, d.n_sm, classes[c], c, false, p.ord.size()));
+        p.ord.insert(p.ord.end(), classes[c].begin(), classes[c].end());
+    }
+    plan_chunks(g, d, k, p);
+    return p;
 }
 
 
@@ -1005,19 +1373,17 @@ int b2c_decoder_create(const char* const* labels, int n_labels, int is_bpe, b2c_
     }
     if (!have_blank) return fail(B2C_E_ARG, "labels must contain the CTC blank \"\" (pass Alphabet.labels)");
     CUDA_OK(cudaSetDevice(device));
-    CUDA_OK(cudaStreamCreate(&d->stream));
-    for (int i = 0; i < 6; ++i) CUDA_OK(cudaEventCreate(&d->ev[i]));
-    for (int i = 0; i < 5; ++i) {
-        CUDA_OK(cudaStreamCreate(&d->cls_stream[i]));
-        CUDA_OK(cudaEventCreate(&d->cls_done[i]));
-    }
-    CUDA_OK(cudaEventCreate(&d->fork_ev));
-    CUDA_OK(cudaEventCreateWithFlags(&d->caller_ev, cudaEventDisableTiming));
-    CUDA_OK(cudaStreamCreate(&d->copy_stream));
-    CUDA_OK(cudaStreamCreate(&d->prep_stream));
-    for (int i = 0; i < 3; ++i) CUDA_OK(cudaEventCreateWithFlags(&d->prep_ev[i], cudaEventDisableTiming));
-    for (int i = 0; i < B2C_PIPE_CHUNKS; ++i) CUDA_OK(cudaEventCreateWithFlags(&d->copied[i], cudaEventDisableTiming));
-    for (int i = 0; i < 3 * B2C_PIPE_CHUNKS; ++i) CUDA_OK(cudaEventCreate(&d->chunk_ev[i]));
+    CUDA_OK(cudaStreamCreate(&d->stream.h));
+    for (Event& e : d->ev) CUDA_OK(cudaEventCreate(&e.h));
+    for (Stream& s : d->cls_stream) CUDA_OK(cudaStreamCreate(&s.h));
+    for (Event& e : d->cls_done) CUDA_OK(cudaEventCreate(&e.h));
+    CUDA_OK(cudaEventCreate(&d->fork_ev.h));
+    CUDA_OK(cudaEventCreateWithFlags(&d->caller_ev.h, cudaEventDisableTiming));
+    CUDA_OK(cudaStreamCreate(&d->copy_stream.h));
+    CUDA_OK(cudaStreamCreate(&d->prep_stream.h));
+    for (Event& e : d->prep_ev) CUDA_OK(cudaEventCreateWithFlags(&e.h, cudaEventDisableTiming));
+    for (Event& e : d->copied) CUDA_OK(cudaEventCreateWithFlags(&e.h, cudaEventDisableTiming));
+    for (Event& e : d->chunk_ev) CUDA_OK(cudaEventCreate(&e.h));
     int v = 0;
     CUDA_OK(cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, device));
     d->n_sm = v;
@@ -1059,27 +1425,7 @@ void b2c_decoder_destroy(b2c_decoder_t* d) {
     if (!d) return;
     cudaSetDevice(d->device);
     if (d->stream) cudaStreamSynchronize(d->stream);
-    DevBuf* bufs[] = {&d->d_raw, &d->d_lmx, &d->d_stream, &d->d_mstats, &d->d_sumk, &d->d_clk, &d->d_maxk, &d->d_toks, &d->d_logits, &d->d_meta, &d->d_tok_start, &d->d_tok_ids, &d->d_tok_lp, &d->d_rowsum, &d->d_set,
-                      &d->d_isprob, &d->d_approx, &d->d_ws, &d->d_hot, &d->d_states, &d->d_out_small, &d->d_out_toks, &d->d_out_frames};
-    for (DevBuf* b : bufs) b->release();
-    PinBuf* pins[] = {&d->h_sumk, &d->h_maxk, &d->h_meta, &d->h_out_small, &d->h_out_toks, &d->h_out_frames, &d->h_mstats};
-    for (PinBuf* b : pins) b->release();
-    for (int i = 0; i < 6; ++i) if (d->ev[i]) cudaEventDestroy(d->ev[i]);
-    for (int i = 0; i < 5; ++i) {
-        if (d->cls_stream[i]) cudaStreamDestroy(d->cls_stream[i]);
-        if (d->cls_done[i]) cudaEventDestroy(d->cls_done[i]);
-    }
-    if (d->fork_ev) cudaEventDestroy(d->fork_ev);
-    if (d->caller_ev) cudaEventDestroy(d->caller_ev);
-    if (d->copy_stream) cudaStreamDestroy(d->copy_stream);
-    if (d->prep_stream) cudaStreamDestroy(d->prep_stream);
-    for (int i = 0; i < 3; ++i) if (d->prep_ev[i]) cudaEventDestroy(d->prep_ev[i]);
-    d->d_gate.release();
-    for (int i = 0; i < B2C_PIPE_CHUNKS; ++i) if (d->copied[i]) cudaEventDestroy(d->copied[i]);
-    for (int i = 0; i < 3 * B2C_PIPE_CHUNKS; ++i) if (d->chunk_ev[i]) cudaEventDestroy(d->chunk_ev[i]);
-    d->d_state.release();
-    if (d->stream) cudaStreamDestroy(d->stream);
-    delete d;
+    delete d;      // buffers, streams and events release themselves
 }
 
 int b2c_decoder_device(const b2c_decoder_t* d) { return d ? d->device : -1; }
@@ -1114,126 +1460,70 @@ void b2c_decode_opts_default(b2c_decode_opts_t* o) {
     o->max_out_beams = 1;
 }
 
-static int decode_batch_locked(b2c_decoder_t* d, const void* const* logits, const int32_t* T, int n_utts, int dtype, int is_device,
-                               const b2c_decode_opts_t* opts, b2c_result_t** out, bool allow_pipe);
-
-int b2c_decode_batch(b2c_decoder_t* d, const void* const* logits, const int32_t* T, int n_utts, int dtype, int is_device,
-                     const b2c_decode_opts_t* opts, b2c_result_t** out) {
-    if (!d || !opts || !out || n_utts < 0 || (n_utts > 0 && (!logits || !T))) return fail(B2C_E_ARG, "null argument");
-    std::lock_guard<std::mutex> call_lock(d->call_mu);      // one call at a time per handle (any number of threads may call)
-    int rc = decode_batch_locked(d, logits, T, n_utts, dtype, is_device, opts, out, true);
-    // a pipelined attempt that could not be planned, or that met probability input (decided after the fact): plain call
-    if (rc == B2C_E_RETRY_PLAIN) rc = decode_batch_locked(d, logits, T, n_utts, dtype, is_device, opts, out, false);
-    return rc;
+// ---- decode call, stage by stage ----------------------------------------------------------------------------
+// batch geometry: frame offsets, longest-first order
+static int set_geometry(Call& c) {
+    Geometry& g = c.g;
+    c.frame_off.resize(g.n_utts);
+    for (int i = 0; i < g.n_utts; ++i) {
+        if (c.T[i] < 0) return fail(B2C_E_ARG, "negative T");
+        if (c.T[i] > 0 && !c.logits[i]) return fail(B2C_E_ARG, "null logits pointer");
+        c.frame_off[i] = g.total_frames;
+        g.total_frames += static_cast<u64>(c.T[i]);
+        g.T_max = std::max(g.T_max, static_cast<int>(c.T[i]));
+    }
+    c.order.resize(g.n_utts); std::iota(c.order.begin(), c.order.end(), 0);
+    const int32_t* T = c.T;
+    std::stable_sort(c.order.begin(), c.order.end(), [T](int a, int b) { return T[a] > T[b]; });
+    g.order = c.order.data();
+    c.OB = std::max(1, std::min(c.opts->max_out_beams, c.opts->beam_width));
+    return 0;
 }
 
-static int decode_batch_locked(b2c_decoder_t* d, const void* const* logits, const int32_t* T, int n_utts, int dtype, int is_device,
-                               const b2c_decode_opts_t* opts, b2c_result_t** out, bool allow_pipe) {
-    if (dtype < B2C_DTYPE_F32 || dtype > B2C_DTYPE_BF16) return fail(B2C_E_ARG, "dtype must be one of B2C_DTYPE_F32 / F64 / F16 / BF16");
-    // half-precision input: copied as 2-byte elements, widened on the device, then the float32 path
-    const int dtype_in = dtype;
-    const bool half_in = dtype_in == B2C_DTYPE_F16 || dtype_in == B2C_DTYPE_BF16;
-    if (half_in) dtype = B2C_DTYPE_F32;
-    d->last_T.clear();
-    if (opts->beam_width < 1) return fail(B2C_E_ARG, "beam_width must be >= 1");
-    if (opts->beam_width > 65535) return fail(B2C_E_ARG, "beam_width above 65535 is not supported");
-    std::unique_ptr<b2c_result> res(new b2c_result());
-    res->utts.resize(n_utts);
-    res->has_lm = d->lm != nullptr;
-    // opt-in host-side section timing (B200CTC_HOST_PROFILE=1, stderr)
-    static const bool host_prof = std::getenv("B200CTC_HOST_PROFILE") != nullptr;
-    auto hp_t0 = std::chrono::steady_clock::now();
-    double hp_ms[6] = {0, 0, 0, 0, 0, 0};
-    auto hp_mark = [&](int k) {
-        const auto now = std::chrono::steady_clock::now();
-        hp_ms[k] += std::chrono::duration<double, std::milli>(now - hp_t0).count();
-        hp_t0 = now;
-    };
-    if (n_utts == 0) { *out = res.release(); return 0; }
-    CUDA_OK(cudaSetDevice(d->device));
-    const int V = d->V;
-    const size_t esz = dtype == B2C_DTYPE_F32 ? 4 : 8;
-    const size_t esz_in = half_in ? 2 : esz;         // element size of the caller's matrices
-    std::memset(&d->tm, 0, sizeof(d->tm));
-
-    // ---- batch geometry -------------------------------------------------------------------
-    std::vector<u64> frame_off(n_utts);
-    u64 total_frames = 0;
-    int T_max = 0;
-    for (int i = 0; i < n_utts; ++i) {
-        if (T[i] < 0) return fail(B2C_E_ARG, "negative T");
-        if (T[i] > 0 && !logits[i]) return fail(B2C_E_ARG, "null logits pointer");
-        frame_off[i] = total_frames;
-        total_frames += static_cast<u64>(T[i]);
-        T_max = std::max(T_max, static_cast<int>(T[i]));
-    }
-    std::vector<int> order(n_utts);
-    std::iota(order.begin(), order.end(), 0);
-    std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return T[a] > T[b]; });
-    const int OB = std::max(1, std::min(opts->max_out_beams, opts->beam_width));
-    // ---- streaming input (partial_decode_beams): flatten the per-utterance beam / word lists -----------
-    if (opts->finalize_mode < B2C_FIN_EOS || opts->finalize_mode > B2C_FIN_KEEP) return fail(B2C_E_ARG, "bad finalize_mode");
-    const bool streaming = opts->stream_states != nullptr || opts->finalize_mode != B2C_FIN_EOS;
-    std::vector<B2cStreamUtt> s_utts;
-    std::vector<B2cStreamBeam> s_beams;
-    std::vector<u64> s_wh;
-    std::vector<u32> s_wl;
-    int s_max_beams = 0;
-    u64 s_max_words = 0;
-    if (opts->stream_states) {
-        s_utts.resize(n_utts);
-        for (int i = 0; i < n_utts; ++i) {
-            const b2c_stream_state_t& ss = opts->stream_states[i];
+// streaming input (partial_decode_beams): flatten the per-utterance beam / word lists
+static int flatten_stream_states(const b2c_decoder* d, Call& c) {
+    const b2c_decode_opts_t* o = c.opts;
+    Geometry& g = c.g;
+    if (o->finalize_mode < B2C_FIN_EOS || o->finalize_mode > B2C_FIN_KEEP) return fail(B2C_E_ARG, "bad finalize_mode");
+    g.streaming = o->stream_states != nullptr || o->finalize_mode != B2C_FIN_EOS;
+    c.text_only = o->text_only != 0 && !g.streaming;
+    if (o->stream_states) {
+        c.s_utts.resize(g.n_utts);
+        for (int i = 0; i < g.n_utts; ++i) {
+            const b2c_stream_state_t& ss = o->stream_states[i];
             if (ss.n_beams < 0 || ss.n_beams > 65535 || (ss.n_beams > 0 && !ss.beams)) return fail(B2C_E_ARG, "bad stream state");
-            B2cStreamUtt su;
-            su.beam_off = static_cast<u32>(s_beams.size());
-            su.n_beams = static_cast<u32>(ss.n_beams);
-            su.t0 = ss.processed_frames;
-            su.pad = 0;
-            const u32 wbase = static_cast<u32>(s_wh.size());
+            const B2cStreamUtt su{static_cast<u32>(c.s_beams.size()), static_cast<u32>(ss.n_beams), ss.processed_frames, 0};
+            const u32 wbase = static_cast<u32>(c.s_wh.size());
             u64 words = 0;
             for (int b = 0; b < ss.n_beams; ++b) {
                 const b2c_stream_beam_t& ib = ss.beams[b];
                 if (static_cast<u64>(ib.word_off) + ib.n_words > static_cast<u64>(std::max(ss.n_words, 0)))
                     return fail(B2C_E_ARG, "stream beam word range outside the state's word list");
-                if (ib.last_tok != B2C_NO_TOK && ib.last_tok >= static_cast<u32>(V)) return fail(B2C_E_ARG, "stream beam last_tok out of range");
-                B2cStreamBeam sb;
-                sb.part_hash = ib.part_hash;
-                sb.logit = ib.logit_score;
-                sb.word_off = wbase + ib.word_off;
-                sb.n_words = ib.n_words;
-                sb.part_len = ib.part_len;
-                sb.last_tok = ib.last_tok == B2C_NO_TOK ? B2C_NO_TOK : d->toks[ib.last_tok].canon;
-                sb.pf_s = ib.pf_s;
-                sb.pf_e = ib.pf_e;
-                s_beams.push_back(sb);
+                if (ib.last_tok != B2C_NO_TOK && ib.last_tok >= static_cast<u32>(g.V)) return fail(B2C_E_ARG, "stream beam last_tok out of range");
+                const u32 last = ib.last_tok == B2C_NO_TOK ? B2C_NO_TOK : d->toks[ib.last_tok].canon;
+                c.s_beams.push_back(B2cStreamBeam{ib.part_hash, ib.logit_score, wbase + ib.word_off, ib.n_words, ib.part_len, last, ib.pf_s, ib.pf_e});
                 words += ib.n_words;
             }
-            for (int w = 0; w < ss.n_words; ++w) { s_wh.push_back(ss.word_hashes[w]); s_wl.push_back(ss.word_lens[w]); }
-            s_utts[i] = su;
-            s_max_beams = std::max(s_max_beams, ss.n_beams);
-            s_max_words = std::max(s_max_words, words);
+            for (int w = 0; w < ss.n_words; ++w) { c.s_wh.push_back(ss.word_hashes[w]); c.s_wl.push_back(ss.word_lens[w]); }
+            c.s_utts[i] = su;
+            g.s_max_beams = std::max(g.s_max_beams, ss.n_beams);
+            g.s_max_words = std::max(g.s_max_words, words);
         }
     }
-    const int W_tab = std::max(opts->beam_width, s_max_beams);     // capacity of the beam tables
+    g.W_tab = std::max(o->beam_width, g.s_max_beams);     // capacity of the beam tables
+    return 0;
+}
 
-    // ---- parameters -----------------------------------------------------------------------
-    B2cParams P;
-    std::memset(&P, 0, sizeof(P));
-    P.V = V;
-    P.is_bpe = d->is_bpe;
-    P.has_dup_labels = d->has_dup_labels;
-    P.beam_width = opts->beam_width;
-    P.prune_history = opts->prune_history ? 1 : 0;
-    P.out_beams = OB;
-    P.narrow_chain = (opts->text_only != 0 && !streaming) ? 1 : 0;
-    P.prune_logp = opts->beam_prune_logp;
-    P.token_min_logp = opts->token_min_logp;
+// kernel parameters, the extra language models of a MultiLanguageModel, the hotword table
+static int make_params(b2c_decoder* d, Call& c) {
+    const b2c_decode_opts_t* o = c.opts;
+    B2cParams& P = c.P;
+    P.V = c.g.V; P.is_bpe = d->is_bpe; P.has_dup_labels = d->has_dup_labels;
+    P.beam_width = o->beam_width; P.prune_history = o->prune_history ? 1 : 0; P.out_beams = c.OB; P.narrow_chain = c.text_only ? 1 : 0;
+    P.prune_logp = o->beam_prune_logp; P.token_min_logp = o->token_min_logp;
     P.alpha = d->alpha; P.beta = d->beta; P.unk_offset = d->unk;
     P.log_base_change = 0x1.26bb1bbb55516p+1;  // 1.0 / math.log10(math.e) (constants.py:18)
-    P.score_boundary = d->score_boundary;
-    P.hot_weight = opts->hotword_weight;
-    P.bucket_scale = b2c_bucket_scale(opts->beam_prune_logp);
+    P.score_boundary = d->score_boundary; P.hot_weight = o->hotword_weight; P.bucket_scale = b2c_bucket_scale(o->beam_prune_logp);
     P.toks = d->d_toks.as<B2cTok>();
     if (d->lm) {
         auto it = d->lm->dev.find(d->device);
@@ -1252,10 +1542,7 @@ static int decode_batch_locked(b2c_decoder_t* d, const void* const* logits, cons
         std::memset(&X, 0, sizeof(X));
         X.lm = x.lm->host.view(it->second);
         if (X.lm.order > B2C_MAX_ORDER) return fail(B2C_E_ARG, "n-gram order too large");
-        X.alpha = x.alpha;
-        X.beta = x.beta;
-        X.unk_offset = x.unk;
-        X.score_boundary = x.score_boundary;
+        X.alpha = x.alpha; X.beta = x.beta; X.unk_offset = x.unk; X.score_boundary = x.score_boundary;
         max_order = std::max(max_order, X.lm.order);
     }
     if (!lmx_host.empty()) {
@@ -1263,888 +1550,600 @@ static int decode_batch_locked(b2c_decoder_t* d, const void* const* logits, cons
         CUDA_OK(cudaMemcpy(d->d_lmx.p, lmx_host.data(), sizeof(B2cLmExtra) * lmx_host.size(), cudaMemcpyHostToDevice));
         P.lmx = d->d_lmx.as<B2cLmExtra>();
     }
-    const int n_lm = std::max(1, P.n_lm);
-    res->n_models = n_lm;
-    res->streaming = streaming;
+    c.g.n_lm = std::max(1, P.n_lm);
     P.hist_n = std::max(1, max_order - 1);
-    std::vector<B2cHot> hot;
-    build_hot(opts, hot, P.n_hot, P.hot_min_len_all);
-    if (d->d_hot.ensure(hot.size() * sizeof(B2cHot))) return B2C_E_NOMEM;
-    P.hot = d->d_hot.as<B2cHot>();
-    P.hot_mask = hot.size() - 1;
+    build_hot(o, c.hot, P.n_hot, P.hot_min_len_all);
+    if (d->d_hot.ensure(c.hot.size() * sizeof(B2cHot))) return B2C_E_NOMEM;
+    P.hot = d->d_hot.as<B2cHot>(); P.hot_mask = c.hot.size() - 1;
+    return 0;
+}
 
-    // ---- buffers --------------------------------------------------------------------------
-    const u64 n_entries = std::max<u64>(total_frames * static_cast<u64>(V), 1);
-    const bool contiguous_dev = [&]() {
-        if (!is_device) return false;
-        for (int i = 0; i + 1 < n_utts; ++i) {
-            if (T[i + 1] == 0) continue;
-            const char* expect = static_cast<const char*>(logits[0]) + frame_off[i + 1] * V * esz_in;
-            if (static_cast<const char*>(logits[i + 1]) != expect) return false;
+static bool contiguous_on_device(const Call& c) {
+    if (!c.is_device) return false;
+    for (int i = 0; i + 1 < c.g.n_utts; ++i) {
+        if (c.T[i + 1] == 0) continue;
+        const char* expect = static_cast<const char*>(c.logits[0]) + c.frame_off[i + 1] * c.g.V * c.esz_in;
+        if (static_cast<const char*>(c.logits[i + 1]) != expect) return false;
+    }
+    return c.T[0] > 0 || c.g.n_utts == 1;
+}
+
+// scratch and output buffers of the call
+static int size_buffers(b2c_decoder* d, Call& c) {
+    Geometry& g = c.g;
+    const int n = g.n_utts, V = g.V;
+    const u64 n_entries = std::max<u64>(g.total_frames * static_cast<u64>(V), 1);
+    c.contiguous_dev = contiguous_on_device(c);
+    if ((c.half_in || !c.contiguous_dev) && d->d_logits.ensure(std::max<u64>(g.total_frames * V * g.esz, 16))) return B2C_E_NOMEM;
+    if (c.half_in && !c.contiguous_dev && d->d_raw.ensure(std::max<u64>(g.total_frames * V * c.esz_in, 16))) return B2C_E_NOMEM;
+    c.meta = MetaLayout(n);
+    if (d->d_meta.ensure(c.meta.bytes) || d->h_meta.ensure(c.meta.bytes)) return B2C_E_NOMEM;
+    if (d->d_tok_start.ensure(sizeof(B2cFrameRec) * (g.total_frames + 1)) || d->d_tok_ids.ensure(4 * n_entries) ||
+        d->d_tok_lp.ensure(8 * n_entries) || d->d_rowsum.ensure(std::max<u64>(8 * g.total_frames, 16)) ||
+        d->d_isprob.ensure(4ull * n) || d->d_approx.ensure(16ull * n + 16))
+        return B2C_E_NOMEM;
+    while (c.set_cap < 8u * (static_cast<u32>(V) + 1)) c.set_cap <<= 1;
+    c.runs_per_utt = std::max(1, (g.T_max + B2C_RUN - 1) / B2C_RUN);
+    c.tiles_per_utt = std::max(1, (g.T_max + B2C_TILE_ROWS - 1) / B2C_TILE_ROWS);
+    const int grid_tok = grid_of(d, static_cast<u64>(n) * c.runs_per_utt, B2C_PREP_WARPS);
+    if (V > 32 && d->d_set.ensure(2ull * c.set_cap * 2 * B2C_PREP_WARPS * grid_tok)) return B2C_E_NOMEM;
+    if (d->d_maxk.ensure(4ull * n) || d->h_maxk.ensure(4ull * n) || d->d_sumk.ensure(4ull * n) || d->h_sumk.ensure(4ull * n))
+        return B2C_E_NOMEM;
+    g.smem_budget = static_cast<u32>(std::min<size_t>(d->smem_optin, 200 * 1024));
+    c.out = OutLayout(n, c.OB, g.n_lm, g.streaming);
+    c.tok_bytes = 4ull * c.OB * (g.total_frames + n); c.frm_bytes = 2 * c.tok_bytes;
+    if (d->d_out_small.ensure(c.out.bytes) || d->h_out_small.ensure(c.out.bytes) || d->d_out_toks.ensure(c.tok_bytes) ||
+        d->h_out_toks.ensure(c.tok_bytes) || d->d_out_frames.ensure(c.frm_bytes) || d->h_out_frames.ensure(c.frm_bytes))
+        return B2C_E_NOMEM;
+    if (c.opts->lm_start_states && d->d_states.ensure(sizeof(B2cLmState) * static_cast<u64>(n) * g.n_lm)) return B2C_E_NOMEM;
+    return 0;
+}
+
+// Pipelined call?  Host input in one [B, T, V] float32 block, alphabet of the lane-per-row streaming kernel, every utterance
+// resident in the latency-first beam kernel (known from the previous call of the same configuration): the batch
+// is cut into chunks along T; chunk c+1 crosses PCIe while chunk c goes through the streaming stage and the beam
+// kernel (chunked launches, state parked in HBM in between).  The launch plan cannot wait for this call's token
+// statistics then: it is made from the hint alone.  Probabilities-vs-logits is decided after the last chunk; a
+// call that turns out to hold probabilities is redone as a plain call (B2C_E_RETRY_PLAIN).
+static int choose_pipelined(b2c_decoder* d, Call& c) {
+    Geometry& g = c.g;
+    g.hint_ok = d->hint_valid && d->hint_beam == g.beam_width && d->hint_lm == (c.P.lm.order > 0 ? 1 : 0) &&
+                d->hint_hot == (c.P.n_hot > 0 ? 1 : 0) && d->hint_prune == c.P.prune_history && d->hint_frames > 0;
+    bool pipe = c.allow_pipe && !c.k.no_pipe && !c.is_device && !c.half_in && g.T_max >= 8 * B2C_TILE_ROWS &&
+                !g.streaming && g.n_lm == 1 && g.beam_width <= 128 && g.hint_ok && !d->pipe_refused;
+    for (int i = 0; i < g.n_utts && pipe; ++i)
+        pipe = c.T[i] == g.T_max && static_cast<const char*>(c.logits[i]) == static_cast<const char*>(c.logits[0]) + static_cast<u64>(i) * g.T_max * g.V * c.esz_in;
+    g.pipelined = pipe;
+    if (!g.hint_ok) { d->pipe_refused = false; d->hinted_refused = false; d->hinted_calls = 0; }   // another configuration: start over
+    if (pipe && d->d_logits.ensure(std::max<u64>(g.total_frames * g.V * g.esz, 16))) return B2C_E_NOMEM;
+    return 0;
+}
+
+// the logits as the streaming stage reads them: in place (one device block), packed by one gather launch, or copied in
+// runs of adjacent utterances (half precision: copied as they are, then widened); pipelined calls copy them chunk by chunk
+static int upload_logits(b2c_decoder* d, Call& c) {
+    const int n = c.g.n_utts, V = c.g.V;
+    if (c.g.pipelined) { c.d_logits = d->d_logits.p; return 0; }
+    if (c.contiguous_dev && !c.half_in) { c.d_logits = c.logits[0]; return 0; }
+    c.d_logits = d->d_logits.p;
+    if (c.is_device && n > 4 && !c.half_in) {
+        const int rc = launch_gather(d, c);
+        if (rc != B2C_NO_GATHER) return rc;
+    }
+    const void* packed_half = c.contiguous_dev ? c.logits[0] : d->d_raw.p;      // half input only
+    char* dst = c.half_in ? d->d_raw.as<char>() : d->d_logits.as<char>();
+    // coalesce runs of utterances that are adjacent in the source into one copy
+    int i = 0;
+    while (i < n && !(c.half_in && c.contiguous_dev)) {
+        if (c.T[i] == 0) { ++i; continue; }
+        int j = i;
+        u64 bytes = static_cast<u64>(c.T[i]) * V * c.esz_in;
+        while (j + 1 < n && c.T[j + 1] > 0 && static_cast<const char*>(c.logits[j + 1]) == static_cast<const char*>(c.logits[i]) + bytes) {
+            ++j;
+            bytes += static_cast<u64>(c.T[j]) * V * c.esz_in;
         }
-        return T[0] > 0 || n_utts == 1;
-    }();
-    if ((half_in || !contiguous_dev) && d->d_logits.ensure(std::max<u64>(total_frames * V * esz, 16))) return B2C_E_NOMEM;
-    if (half_in && !contiguous_dev && d->d_raw.ensure(std::max<u64>(total_frames * V * esz_in, 16))) return B2C_E_NOMEM;
-    const size_t meta_bytes = al16(8ull * n_utts) + 3 * al16(4ull * n_utts) + 64 + al16(8ull * (n_utts + 1)) + al16(8ull * n_utts);
-    if (d->d_meta.ensure(meta_bytes) || d->h_meta.ensure(meta_bytes)) return B2C_E_NOMEM;
-    if (d->d_tok_start.ensure(sizeof(B2cFrameRec) * (total_frames + 1)) || d->d_tok_ids.ensure(4 * n_entries) ||
-        d->d_tok_lp.ensure(8 * n_entries) || d->d_rowsum.ensure(std::max<u64>(8 * total_frames, 16)) ||
-        d->d_isprob.ensure(4ull * n_utts) || d->d_approx.ensure(16ull * n_utts + 16))
-        return B2C_E_NOMEM;
-    u32 set_cap = 16;
-    while (set_cap < 8u * (static_cast<u32>(V) + 1)) set_cap <<= 1;
-    std::vector<u64> run_off(n_utts + 1, 0);
-    for (int i = 0; i < n_utts; ++i) run_off[i + 1] = run_off[i] + (static_cast<u64>(T[i]) + B2C_RUN - 1) / B2C_RUN;
-    const int runs_per_utt = std::max(1, (T_max + B2C_RUN - 1) / B2C_RUN);
-    const u64 total_runs = static_cast<u64>(n_utts) * runs_per_utt;
-    const int tiles_per_utt = std::max(1, (T_max + B2C_TILE_ROWS - 1) / B2C_TILE_ROWS);
-    const int grid_tile = static_cast<int>(std::max<u64>(1, std::min<u64>((static_cast<u64>(n_utts) * tiles_per_utt + B2C_TILE_WARPS - 1) / B2C_TILE_WARPS, static_cast<u64>(d->n_sm) * 8)));
-    const int grid_tok = static_cast<int>(std::max<u64>(1, std::min<u64>((total_runs + B2C_PREP_WARPS - 1) / B2C_PREP_WARPS, static_cast<u64>(d->n_sm) * 8)));
-    if (V > 32) {
-        if (d->d_set.ensure(2ull * set_cap * 2 * B2C_PREP_WARPS * grid_tok)) return B2C_E_NOMEM;
+        CUDA_OK(cudaMemcpyAsync(dst + c.frame_off[i] * V * c.esz_in, c.logits[i], bytes,
+                                c.is_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, d->stream));
+        if (!c.is_device) d->tm.h2d_bytes += static_cast<long long>(bytes);
+        i = j + 1;
     }
-    if (d->d_maxk.ensure(4ull * n_utts) || d->h_maxk.ensure(4ull * n_utts) || d->d_sumk.ensure(4ull * n_utts) ||
-        d->h_sumk.ensure(4ull * n_utts))
-        return B2C_E_NOMEM;
-    const u32 smem_budget = static_cast<u32>(std::min<size_t>(d->smem_optin, 200 * 1024));
-    // outputs
-    const u64 off_nb = 0, off_st = al16(4ull * n_utts), off_sc = off_st + al16(4ull * n_utts),
-              off_nt = off_sc + al16(16ull * OB * n_utts), off_nw = off_nt + al16(4ull * OB * n_utts),
-              off_ls = off_nw + al16(4ull * OB * n_utts), off_ax = off_ls + al16(sizeof(B2cLmState) * static_cast<u64>(OB) * n_utts),
-              off_lx = off_ax + (streaming ? al16(16ull * OB * n_utts) : 0),
-              small_bytes = off_lx + al16(sizeof(B2cLmState) * static_cast<u64>(OB) * n_utts * static_cast<u64>(n_lm - 1));
-    const u64 tok_bytes = 4ull * OB * (total_frames + n_utts), frm_bytes = 2 * tok_bytes;
-    if (d->d_out_small.ensure(small_bytes) || d->h_out_small.ensure(small_bytes) || d->d_out_toks.ensure(tok_bytes) ||
-        d->h_out_toks.ensure(tok_bytes) || d->d_out_frames.ensure(frm_bytes) || d->h_out_frames.ensure(frm_bytes))
-        return B2C_E_NOMEM;
-    if (opts->lm_start_states) {
-        if (d->d_states.ensure(sizeof(B2cLmState) * static_cast<u64>(n_utts) * n_lm)) return B2C_E_NOMEM;
-    }
+    if (c.half_in && c.g.total_frames > 0)
+        B2C_TRY(launch_widen(d, static_cast<const u16*>(packed_half), d->d_logits.as<float>(), c.g.total_frames * static_cast<u64>(V),
+                             c.dtype_in == B2C_DTYPE_BF16 ? 1 : 0, d->stream));
+    return 0;
+}
 
-    // ---- pipelined call? ---------------------------------------------------------------------
-    // Host input in one [B, T, V] float32 block, alphabet of the lane-per-row streaming kernel, every utterance
-    // resident in the latency-first beam kernel (known from the previous call of the same configuration): the batch
-    // is cut into chunks along T; chunk c+1 crosses PCIe while chunk c goes through the streaming stage and the beam
-    // kernel (chunked launches, state parked in HBM in between).  The launch plan cannot wait for this call's token
-    // statistics then: it is made from the hint alone.  Probabilities-vs-logits is decided after the last chunk; a
-    // call that turns out to hold probabilities is redone as a plain call (B2C_E_RETRY_PLAIN).
-    const bool hint_ok = d->hint_valid && d->hint_beam == opts->beam_width && d->hint_lm == (P.lm.order > 0 ? 1 : 0) &&
-                         d->hint_hot == (P.n_hot > 0 ? 1 : 0) && d->hint_prune == P.prune_history && d->hint_frames > 0;
-    const bool no_pipe = std::getenv("B200CTC_NO_PIPELINE") != nullptr || !env_switch("B200CTC_PIPELINE", B2C_DEFAULT_PIPELINE != 0);
-    bool pipe_candidate = allow_pipe && !no_pipe && !is_device && !half_in && T_max >= 8 * B2C_TILE_ROWS &&
-                          !streaming && n_lm == 1 && opts->beam_width <= 128 && hint_ok && !d->pipe_refused;
-    for (int i = 0; i < n_utts && pipe_candidate; ++i)
-        pipe_candidate = T[i] == T_max && static_cast<const char*>(logits[i]) == static_cast<const char*>(logits[0]) + static_cast<u64>(i) * T_max * V * esz_in;
-    if (!hint_ok) d->pipe_refused = false;                       // another configuration: a new attempt may be planned
-    if (!hint_ok) { d->hinted_refused = false; d->hinted_calls = 0; }
-    static const bool no_hinted = std::getenv("B200CTC_NO_HINTED") != nullptr;
-    if (pipe_candidate && d->d_logits.ensure(std::max<u64>(total_frames * V * esz, 16))) return B2C_E_NOMEM;
-    const int chunk_len = ((T_max + B2C_PIPE_CHUNKS * B2C_TILE_ROWS - 1) / (B2C_PIPE_CHUNKS * B2C_TILE_ROWS)) * B2C_TILE_ROWS;
-
-    // ---- host -> device -------------------------------------------------------------------
+// host -> device: metadata, logits, hotword table, LM start states, streaming states
+static int upload(b2c_decoder* d, Call& c) {
+    const int n = c.g.n_utts;
     cudaStream_t st = d->stream;
     CUDA_OK(cudaEventRecord(d->ev[0], st));
-    u8* hm = d->h_meta.as<u8>();
-    u64* h_fo = reinterpret_cast<u64*>(hm);
-    int* h_T = reinterpret_cast<int*>(hm + al16(8ull * n_utts));
-    const size_t off_run = al16(8ull * n_utts) + al16(4ull * n_utts);
-    const size_t off_ord = off_run + al16(8ull * (n_utts + 1));
-    const size_t off_next = off_ord + 2 * al16(4ull * n_utts);
-    const size_t off_ptr = off_next + 64;                        // [n_utts] source pointers (gather launch only)
-    u64* h_run = reinterpret_cast<u64*>(hm + off_run);
-    for (int i = 0; i <= n_utts; ++i) h_run[i] = run_off[i];
-    int* h_ord = reinterpret_cast<int*>(hm + off_ord);           // [2 * n_utts]: class lists, then retry list
-    u32* h_next = reinterpret_cast<u32*>(hm + off_next);         // [16] one queue head per launch
-    for (int i = 0; i < n_utts; ++i) { h_fo[i] = frame_off[i]; h_T[i] = T[i]; }
-    CUDA_OK(cudaMemcpyAsync(d->d_meta.p, hm, off_ord, cudaMemcpyHostToDevice, st));
-    u8* dm = d->d_meta.as<u8>();
-    const u64* d_fo = reinterpret_cast<const u64*>(dm);
-    const int* d_T = reinterpret_cast<const int*>(dm + al16(8ull * n_utts));
-    int* d_ord = reinterpret_cast<int*>(dm + off_ord);
-    u32* d_next = reinterpret_cast<u32*>(dm + off_next);
-    d->tm.h2d_bytes += static_cast<long long>(meta_bytes);
-    const void* d_logits = nullptr;
-    if (pipe_candidate) {
-        d_logits = d->d_logits.p;                    // copied chunk by chunk further down
-    } else if (contiguous_dev && !half_in) {
-        d_logits = logits[0];
-#ifndef B2C_HOSTSIM
-    } else if (is_device && n_utts > 4 && !half_in) {
-        d_logits = d->d_logits.p;
-        const void** h_ptr = reinterpret_cast<const void**>(hm + off_ptr);
-        for (int i = 0; i < n_utts; ++i) h_ptr[i] = logits[i];
-        CUDA_OK(cudaMemcpyAsync(dm + off_ptr, h_ptr, 8ull * n_utts, cudaMemcpyHostToDevice, st));
-        const int chunks = std::max(1, std::min(64, (d->n_sm * 8 + n_utts - 1) / n_utts));
-        b2c_gather_kernel<<<n_utts * chunks, 256, 0, st>>>(reinterpret_cast<const void* const*>(dm + off_ptr), d_fo, d_T,
-                                                         static_cast<u64>(V) * (esz / 4), d->d_logits.as<u32>(), n_utts, chunks);
-        CUDA_OK(cudaGetLastError());
-        d->tm.launches += 1;
-#endif
-    } else {
-        d_logits = d->d_logits.p;
-        const void* packed_half = contiguous_dev ? logits[0] : d->d_raw.p;      // half input only
-        char* dst = half_in ? d->d_raw.as<char>() : d->d_logits.as<char>();
-        // coalesce runs of utterances that are adjacent in the source into one copy
-        int i = 0;
-        while (i < n_utts && !(half_in && contiguous_dev)) {
-            if (T[i] == 0) { ++i; continue; }
-            int j = i;
-            u64 bytes = static_cast<u64>(T[i]) * V * esz_in;
-            while (j + 1 < n_utts && T[j + 1] > 0 &&
-                   static_cast<const char*>(logits[j + 1]) == static_cast<const char*>(logits[i]) + bytes) {
-                ++j;
-                bytes += static_cast<u64>(T[j]) * V * esz_in;
-            }
-            CUDA_OK(cudaMemcpyAsync(dst + frame_off[i] * V * esz_in, logits[i], bytes,
-                                    is_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st));
-            if (!is_device) d->tm.h2d_bytes += static_cast<long long>(bytes);
-            i = j + 1;
-        }
-        if (half_in && total_frames > 0) {
-            const u64 n_el = total_frames * static_cast<u64>(V);
-#ifndef B2C_HOSTSIM
-            const int blocks = static_cast<int>(std::min<u64>((n_el + 255) / 256, static_cast<u64>(d->n_sm) * 16));
-            b2c_widen_kernel<<<blocks, 256, 0, st>>>(static_cast<const u16*>(packed_half), d->d_logits.as<float>(), n_el,
-                                                     dtype_in == B2C_DTYPE_BF16 ? 1 : 0);
-            CUDA_OK(cudaGetLastError());
-#else
-            b2c_widen_range(static_cast<const u16*>(packed_half), d->d_logits.as<float>(), 0, n_el, 1, dtype_in == B2C_DTYPE_BF16 ? 1 : 0);
-#endif
-            d->tm.launches += 1;
-        }
+    c.hm = d->h_meta.as<u8>(); c.dm = d->d_meta.as<u8>();
+    u64 *h_fo = reinterpret_cast<u64*>(c.hm), *h_run = reinterpret_cast<u64*>(c.hm + c.meta.run);
+    int* h_T = reinterpret_cast<int*>(c.hm + c.meta.T);
+    h_run[0] = 0;
+    for (int i = 0; i < n; ++i) {
+        h_fo[i] = c.frame_off[i]; h_T[i] = c.T[i];
+        h_run[i + 1] = h_run[i] + (static_cast<u64>(c.T[i]) + B2C_RUN - 1) / B2C_RUN;
     }
-    CUDA_OK(cudaMemcpyAsync(d->d_hot.p, hot.data(), hot.size() * sizeof(B2cHot), cudaMemcpyHostToDevice, st));
-    const B2cLmState* d_start = nullptr;
-    std::vector<B2cLmState> start_host;
-    if (opts->lm_start_states) {
+    CUDA_OK(cudaMemcpyAsync(c.dm, c.hm, c.meta.ord, cudaMemcpyHostToDevice, st));
+    d->tm.h2d_bytes += static_cast<long long>(c.meta.bytes);
+    B2C_TRY(upload_logits(d, c));
+    CUDA_OK(cudaMemcpyAsync(d->d_hot.p, c.hot.data(), c.hot.size() * sizeof(B2cHot), cudaMemcpyHostToDevice, st));
+    if (c.opts->lm_start_states) {
         // with a MultiLanguageModel: n_lm consecutive states per utterance (MultiLanguageModelState.states)
-        start_host.resize(static_cast<size_t>(n_utts) * n_lm);
-        for (size_t i = 0; i < start_host.size(); ++i) to_internal(opts->lm_start_states + i, start_host[i]);
+        std::vector<B2cLmState> start_host(static_cast<size_t>(n) * c.g.n_lm);
+        for (size_t i = 0; i < start_host.size(); ++i) to_internal(c.opts->lm_start_states + i, start_host[i]);
         CUDA_OK(cudaMemcpyAsync(d->d_states.p, start_host.data(), sizeof(B2cLmState) * start_host.size(), cudaMemcpyHostToDevice, st));
-        d_start = d->d_states.as<B2cLmState>();
+        c.BA.start_states = d->d_states.as<B2cLmState>();
     }
-
-    const B2cStreamUtt* d_sutt = nullptr;
-    const B2cStreamBeam* d_sbeam = nullptr;
-    const u64* d_swh = nullptr;
-    const u32* d_swl = nullptr;
-    if (!s_utts.empty()) {
-        const size_t b0 = al16(sizeof(B2cStreamUtt) * s_utts.size()), b1 = al16(sizeof(B2cStreamBeam) * std::max<size_t>(s_beams.size(), 1)),
-                     b2 = al16(8 * std::max<size_t>(s_wh.size(), 1)), b3 = al16(4 * std::max<size_t>(s_wl.size(), 1));
+    if (!c.s_utts.empty()) {
+        const size_t b0 = al16(sizeof(B2cStreamUtt) * c.s_utts.size()), b1 = al16(sizeof(B2cStreamBeam) * std::max<size_t>(c.s_beams.size(), 1)),
+                     b2 = al16(8 * std::max<size_t>(c.s_wh.size(), 1)), b3 = al16(4 * std::max<size_t>(c.s_wl.size(), 1));
         if (d->d_stream.ensure(b0 + b1 + b2 + b3)) return B2C_E_NOMEM;
         u8* base = d->d_stream.as<u8>();
-        CUDA_OK(cudaMemcpyAsync(base, s_utts.data(), sizeof(B2cStreamUtt) * s_utts.size(), cudaMemcpyHostToDevice, st));
-        if (!s_beams.empty()) CUDA_OK(cudaMemcpyAsync(base + b0, s_beams.data(), sizeof(B2cStreamBeam) * s_beams.size(), cudaMemcpyHostToDevice, st));
-        if (!s_wh.empty()) {
-            CUDA_OK(cudaMemcpyAsync(base + b0 + b1, s_wh.data(), 8 * s_wh.size(), cudaMemcpyHostToDevice, st));
-            CUDA_OK(cudaMemcpyAsync(base + b0 + b1 + b2, s_wl.data(), 4 * s_wl.size(), cudaMemcpyHostToDevice, st));
+        CUDA_OK(cudaMemcpyAsync(base, c.s_utts.data(), sizeof(B2cStreamUtt) * c.s_utts.size(), cudaMemcpyHostToDevice, st));
+        if (!c.s_beams.empty()) CUDA_OK(cudaMemcpyAsync(base + b0, c.s_beams.data(), sizeof(B2cStreamBeam) * c.s_beams.size(), cudaMemcpyHostToDevice, st));
+        if (!c.s_wh.empty()) {
+            CUDA_OK(cudaMemcpyAsync(base + b0 + b1, c.s_wh.data(), 8 * c.s_wh.size(), cudaMemcpyHostToDevice, st));
+            CUDA_OK(cudaMemcpyAsync(base + b0 + b1 + b2, c.s_wl.data(), 4 * c.s_wl.size(), cudaMemcpyHostToDevice, st));
         }
-        d_sutt = reinterpret_cast<const B2cStreamUtt*>(base);
-        d_sbeam = reinterpret_cast<const B2cStreamBeam*>(base + b0);
-        d_swh = reinterpret_cast<const u64*>(base + b0 + b1);
-        d_swl = reinterpret_cast<const u32*>(base + b0 + b1 + b2);
+        c.BA.s_utts = reinterpret_cast<const B2cStreamUtt*>(base); c.BA.s_beams = reinterpret_cast<const B2cStreamBeam*>(base + b0);
+        c.BA.s_word_hash = reinterpret_cast<const u64*>(base + b0 + b1); c.BA.s_word_len = reinterpret_cast<const u32*>(base + b0 + b1 + b2);
         d->tm.h2d_bytes += static_cast<long long>(b0 + b1 + b2 + b3);
     }
+    return 0;
+}
 
-    // ---- prepare kernel ---------------------------------------------------------------------
-    B2cPrepArgs PA;
-    std::memset(&PA, 0, sizeof(PA));
-    PA.logits = d_logits;
-    PA.frame_off = d_fo;
-    PA.T = d_T;
-    PA.V = V;
-    PA.token_min_logp = opts->token_min_logp;
-    PA.run_off = reinterpret_cast<const u64*>(dm + off_run);
-    PA.n_utts = n_utts;
-    PA.total_frames = total_frames;
-    PA.tok_rec = d->d_tok_start.as<B2cFrameRec>();
-    PA.tok_ids = d->d_tok_ids.as<u32>();
-    PA.tok_lp = d->d_tok_lp.as<double>();
-    PA.rowsum = d->d_rowsum.p;
-    PA.set_scratch = d->d_set.as<u16>();
-    PA.set_cap = set_cap;
-    PA.is_prob = d->d_isprob.as<int>();
-    PA.tile_lo = 0;
-    PA.tile_hi = tiles_per_utt;
-    PA.run_lo = 0;
-    PA.run_hi = runs_per_utt;
-    PA.approx = d->d_approx.as<double>();
-    CUDA_OK(cudaMemsetAsync(d->d_approx.p, 0, 16ull * n_utts + 16, st));
-    PA.max_k = d->d_maxk.as<u32>();
-    PA.sum_k = d->d_sumk.as<u32>();
-    CUDA_OK(cudaMemsetAsync(d->d_maxk.p, 0, 4ull * n_utts, st));
-    CUDA_OK(cudaMemsetAsync(d->d_sumk.p, 0, 4ull * n_utts, st));
-    int rc = 0;
-    bool hinted = false;
-    if (!pipe_candidate) {
-        CUDA_OK(cudaEventRecord(d->ev[1], st));
-        rc = dtype == B2C_DTYPE_F32 ? launch_prepare<float>(d, PA, n_utts, grid_tile, grid_tok)
-                                    : launch_prepare<double>(d, PA, n_utts, grid_tile, grid_tok);
-        if (rc) return rc;
-        CUDA_OK(cudaEventRecord(d->ev[2], st));
-        d->tm.launches += 3;
+// the streaming stage (K1): streaming pass (every utterance as logits) -> decide -> second pass over the utterances that
+// turned out to be probabilities.  A plain call then waits for the token statistics -- unless it is hinted: planned from
+// the hint alone, its beam kernel enqueued right behind the streaming stage.  Pipelined calls run K1 chunk by chunk later.
+static int run_streaming_stage(b2c_decoder* d, Call& c) {
+    const Geometry& g = c.g;
+    const int n = g.n_utts;
+    cudaStream_t st = d->stream;
+    B2cPrepArgs& PA = c.PA;
+    PA.logits = c.d_logits;
+    PA.frame_off = reinterpret_cast<const u64*>(c.dm); PA.T = reinterpret_cast<const int*>(c.dm + c.meta.T);
+    PA.run_off = reinterpret_cast<const u64*>(c.dm + c.meta.run);
+    PA.V = g.V; PA.token_min_logp = c.opts->token_min_logp; PA.n_utts = n; PA.total_frames = g.total_frames;
+    PA.tok_rec = d->d_tok_start.as<B2cFrameRec>(); PA.tok_ids = d->d_tok_ids.as<u32>(); PA.tok_lp = d->d_tok_lp.as<double>();
+    PA.rowsum = d->d_rowsum.p; PA.set_scratch = d->d_set.as<u16>(); PA.set_cap = c.set_cap; PA.is_prob = d->d_isprob.as<int>();
+    PA.tile_lo = 0; PA.tile_hi = c.tiles_per_utt; PA.run_lo = 0; PA.run_hi = c.runs_per_utt;
+    PA.approx = d->d_approx.as<double>(); PA.max_k = d->d_maxk.as<u32>(); PA.sum_k = d->d_sumk.as<u32>();
+    CUDA_OK(cudaMemsetAsync(d->d_approx.p, 0, 16ull * n + 16, st));
+    CUDA_OK(cudaMemsetAsync(d->d_maxk.p, 0, 4ull * n, st));
+    CUDA_OK(cudaMemsetAsync(d->d_sumk.p, 0, 4ull * n, st));
+    if (g.pipelined) return 0;
+    CUDA_OK(cudaEventRecord(d->ev[1], st));
+    B2cPrepArgs A1 = PA;               // the second pass
+    A1.mode = 1;
+    B2C_TRY(launch_tokens(d, PA, c.f64, st));
+    B2C_TRY(launch_decide(d, PA, c.f64, st));
+    B2C_TRY(launch_tokens(d, A1, c.f64, st));
+    CUDA_OK(cudaEventRecord(d->ev[2], st));
+    CUDA_OK(cudaMemcpyAsync(d->h_maxk.p, d->d_maxk.p, 4ull * n, cudaMemcpyDeviceToHost, st));
+    CUDA_OK(cudaMemcpyAsync(d->h_sumk.p, d->d_sumk.p, 4ull * n, cudaMemcpyDeviceToHost, st));
+    c.hp.mark(0);                                 // argument checks, buffers, enqueue of H2D + prepare kernels
+    // if the plan is not the one the last statistics-based call ran, a hinted call waits for the statistics after all
+    c.hinted = c.allow_pipe && !c.k.no_hinted && g.hint_ok && !g.streaming && g.n_lm == 1 && g.beam_width <= 128 && d->plain_v5 >= 0 &&
+               (d->hinted_calls++ % 32u) != 31u && !d->hinted_refused;
+    if ((d->hinted_calls % 32u) == 0u) d->hinted_refused = false;       // the refresh call ran: try the hint again
+    if (!c.hinted) {
+        CUDA_OK(cudaStreamSynchronize(st));
+        c.hp.mark(1);                             // wait: H2D + prepare kernels
+    }
+    return 0;
+}
 
-        // ---- size the beam kernel from the token statistics of this batch ---------------------------
-        CUDA_OK(cudaMemcpyAsync(d->h_maxk.p, d->d_maxk.p, 4ull * n_utts, cudaMemcpyDeviceToHost, st));
-        CUDA_OK(cudaMemcpyAsync(d->h_sumk.p, d->d_sumk.p, 4ull * n_utts, cudaMemcpyDeviceToHost, st));
-        hp_mark(0);                                   // argument checks, buffers, enqueue of H2D + prepare kernels
-        // hinted plain call: plan now, from the hint alone, and launch the beam kernel right behind the streaming stage;
-        // if the plan is not the one the last statistics-based call ran, wait for the statistics after all (below)
-        hinted = allow_pipe && !no_hinted && hint_ok && !streaming && n_lm == 1 && opts->beam_width <= 128 && d->plain_v5 >= 0 &&
-                 (d->hinted_calls++ % 32u) != 31u && !d->hinted_refused;
-        if ((d->hinted_calls % 32u) == 0u) d->hinted_refused = false;       // the refresh call ran: try the hint again
-        if (!hinted) {
-            CUDA_OK(cudaStreamSynchronize(st));
-            hp_mark(1);                               // wait: H2D + prepare kernels
-        }
-    }
-    // without this call's statistics (pipelined and hinted calls): the worst case (V tokens in a frame) sizes the
-    // workspace; the capacity class comes from the hint (one token per frame "on average" keeps the statistics-based
-    // bound out of its way)
-    std::vector<u32> nostat_maxk, nostat_sumk;
-    if (pipe_candidate || hinted) {
-        nostat_maxk.assign(n_utts, static_cast<u32>(V));
-        nostat_sumk.resize(n_utts);
-        for (int i = 0; i < n_utts; ++i) nostat_sumk[i] = static_cast<u32>(T[i]);
-    }
-    const u32* h_maxk = nullptr;
-    const u32* h_sumk = nullptr;
-    // ---- capacity class of the shared-memory candidate tier (ONE fast class per call) -------------
-    // upper bound: sized for the TYPICAL frame of an utterance if all beam_width beams were alive
-    // (2.5 x its mean tokens per frame, at least 4); with a hint from the previous call of the same
-    // configuration (histogram of the per-frame candidate counts actually seen -- with an LM far fewer
-    // beams stay alive): the smallest class that covers all but 0.4% of the frames.  The few wider
-    // frames take the out-of-line HBM-tier step inside the same kernel, so every choice is exact.
-    // Small classes run 64-thread CTAs (255 registers x 64 threads: 4 CTAs per SM), the others 128.
-    static const int kNumCaps = 6;
-    static const u32 kCaps[kNumCaps] = {128, 256, 512, 1024, 2048, 4096};
-    // big classes leave room for one CTA per SM only: give that CTA 256 threads (a diffuse frame has ~650 candidates)
-    auto threads_of = [&](int c) { return kCaps[c] <= 128 ? 32 : (kCaps[c] <= 256 ? 64 : (kCaps[c] >= 2048 ? 256 : 128)); };
-    auto layout_of = [&](int c, int tmax, bool full, u64 worst_m) {
-        // the 2048 / 4096-candidate classes own an SM anyway: they rank over the wide bucket array
-        return make_layout(opts->beam_width, V, tmax, full, smem_budget, kCaps[c], worst_m, threads_of(c) / 32, 0, 0, 1,
-                           kCaps[c] >= 2048 ? B2C_NBUCKET_WIDE : B2C_NBUCKET);
-    };
-    auto per_sm_of = [&](u32 smem_bytes, int threads) {
-        const int by_smem = static_cast<int>(std::max<u64>(1, (224 * 1024) / std::max<u32>(smem_bytes + 1024, 2048)));
-        return std::min(by_smem, threads == 32 ? 8 : (threads == 64 ? 4 : (threads >= 256 ? 1 : 2)));
-    };
-    bool cap_ok[kNumCaps];
-    for (int c = 0; c < kNumCaps; ++c) cap_ok[c] = layout_of(c, 1, false, 0).smem_bytes <= smem_budget;
-    std::vector<std::vector<int>> classes;                 // fast classes (one used per call), last = general
-    bool use_v5 = false, use_lean = false;
-    int v5_top = -1, v5_variant = 0;
-    auto classify = [&]() {
-        classes.assign(kNumCaps + 1, std::vector<int>());
-        use_v5 = false; use_lean = false;
-        v5_top = -1; v5_variant = 0;
-        std::vector<int> cls_of(n_utts, kNumCaps);
-        int top = -1, n_fast = 0;
-        for (int u = 0; u < n_utts; ++u) {
-            const double mean_k = T[u] > 0 ? static_cast<double>(h_sumk[u]) / T[u] : 1.0;
-            const u32 typ_k = std::min<u32>(std::max<u32>(h_maxk[u], 1u), std::max<u32>(4u, static_cast<u32>(std::ceil(2.5 * mean_k))));
-            const u64 need = std::min<u64>(static_cast<u64>(opts->beam_width) * typ_k,
-                                           static_cast<u64>(opts->beam_width) * static_cast<u64>(V));
-            for (int c = 0; c < kNumCaps && !streaming && n_lm == 1; ++c)      // streaming / multi-LM calls take the general kernel
-                if (cap_ok[c] && need <= kCaps[c]) { cls_of[u] = c; break; }
-            if (cls_of[u] < kNumCaps) { top = std::max(top, cls_of[u]); ++n_fast; }
-        }
-        if (top >= 0 && hint_ok) {
-            int c_hint = kNumCaps - 1;
-            for (int c = 0; c < kNumCaps; ++c)
-                if (static_cast<double>(d->hint_over[c]) <= 0.004 * d->hint_frames) { c_hint = c; break; }
-            while (c_hint < top && !cap_ok[c_hint]) ++c_hint;
-            top = std::min(top, c_hint);
-        }
-        v5_top = top;                            // the class the statistics ask for, before the residency upgrade
-        // upgrade while every fast utterance stays resident (fewer frames need the out-of-line step)
-        while (top >= 0 && top + 1 < kNumCaps && cap_ok[top + 1]) {
-            const u32 sb = layout_of(top + 1, 1, false, 0).smem_bytes;
-            if (static_cast<long long>(d->n_sm) * per_sm_of(sb, threads_of(top + 1)) < n_fast) break;
-            ++top;
-        }
-        // beam_width <= 128 and a typical frame within 1024 candidates: the latency-first kernel (v5) takes
-        // the whole fast list; wider frames inside it go through its out-of-line HBM-tier step
-        const bool force_v5 = std::getenv("B200CTC_FORCE_V5") != nullptr;      // tests: exercise the out-of-line step
-        use_v5 = top >= 0 && opts->beam_width <= 128 && (force_v5 || kCaps[v5_top >= 0 ? v5_top : top] <= 1024) &&
-                 kV5Smem[0][1] + 1024 <= d->smem_optin && std::getenv("B200CTC_NO_V5") == nullptr;
-        // more utterances than variant A keeps resident: trade capacity for residency if the previous call's
-        // histogram says that all but 0.4% of the frames fit (hint_over[q] = frames with > 128 << q candidates)
-        if (use_v5 && hint_ok && n_fast > d->n_sm * kV5Occ[0] && std::getenv("B200CTC_V5_VARIANT") == nullptr) {
-            for (int v = 2; v >= 1; --v) {
-                const int q = kV5Cap[v] == 256 ? 1 : 2;
-                if (static_cast<double>(d->hint_over[q]) <= 0.004 * d->hint_frames) { v5_variant = v; break; }
-            }
-        }
-        if (const char* e = std::getenv("B200CTC_V5_VARIANT")) v5_variant = std::max(0, std::min(2, std::atoi(e)));
-        // the lean one-warp variant: more utterances than the chosen variant keeps resident, and the previous call of
-        // this configuration says that (nearly) every utterance fits 32 slots / 128 candidates / 16 tokens per frame
-        const bool no_lean = std::getenv("B200CTC_NO_LEAN") != nullptr || !env_switch("B200CTC_LEAN", B2C_DEFAULT_LEAN != 0);
-        const bool force_lean = std::getenv("B200CTC_FORCE_LEAN") != nullptr;
-        use_lean = use_v5 && opts->beam_width <= 128 &&
-                   (force_lean || (!no_lean && (hint_ok && !d->lean_bad && d->hint_utts > 0 && 20ull * d->hint_wide_utts <= d->hint_utts &&
-                                   n_fast > d->n_sm * kV5Occ[v5_variant])));
-        for (int q = 0; q < n_utts; ++q) {
-            const int u = order[q];             // keeps longest-first order inside every class
-            classes[cls_of[u] < kNumCaps ? top : kNumCaps].push_back(u);
-        }
-    };
-    B2cBeamArgs BA;
-    std::memset(&BA, 0, sizeof(BA));
-    BA.P = P;
-    BA.frame_off = d_fo;
-    BA.T = d_T;
-    BA.tok_rec = PA.tok_rec;
-    BA.tok_ids = PA.tok_ids;
-    BA.tok_lp = PA.tok_lp;
-    BA.start_states = d_start;
-    BA.s_utts = d_sutt;
-    BA.s_beams = d_sbeam;
-    BA.s_word_hash = d_swh;
-    BA.s_word_len = d_swl;
-    BA.fin_mode = opts->finalize_mode;
-    u8* ds = d->d_out_small.as<u8>();
-    BA.out_nbeams = reinterpret_cast<int*>(ds + off_nb);
-    BA.out_status = reinterpret_cast<int*>(ds + off_st);
-    BA.out_scores = reinterpret_cast<double*>(ds + off_sc);
-    BA.out_ntok = reinterpret_cast<int*>(ds + off_nt);
-    BA.out_nwords = reinterpret_cast<int*>(ds + off_nw);
-    BA.out_states = reinterpret_cast<B2cLmState*>(ds + off_ls);
-    BA.out_aux = streaming ? reinterpret_cast<int*>(ds + off_ax) : nullptr;
-    BA.out_states_x = n_lm > 1 ? reinterpret_cast<B2cLmState*>(ds + off_lx) : nullptr;
-    BA.out_toks = d->d_out_toks.as<u32>();
-    BA.out_frames = d->d_out_frames.as<int>();
+static int fill_beam_args(b2c_decoder* d, Call& c) {
+    B2cBeamArgs& BA = c.BA;
+    BA.P = c.P;
+    BA.frame_off = c.PA.frame_off; BA.T = c.PA.T; BA.tok_rec = c.PA.tok_rec; BA.tok_ids = c.PA.tok_ids; BA.tok_lp = c.PA.tok_lp;
+    BA.fin_mode = c.opts->finalize_mode;
+    const OutViews o = c.out.at(d->d_out_small.as<u8>());
+    BA.out_nbeams = o.nbeams; BA.out_status = o.status; BA.out_scores = o.scores; BA.out_ntok = o.ntok; BA.out_nwords = o.nwords;
+    BA.out_states = o.states; BA.out_aux = o.aux; BA.out_states_x = o.states_x;
+    BA.out_toks = d->d_out_toks.as<u32>(); BA.out_frames = d->d_out_frames.as<int>();
     if (d->d_mstats.ensure(64)) return B2C_E_NOMEM;
-    CUDA_OK(cudaMemsetAsync(d->d_mstats.p, 0, 64, st));
+    CUDA_OK(cudaMemsetAsync(d->d_mstats.p, 0, 64, d->stream));
     BA.m_stats = d->d_mstats.as<u32>();
 #if defined(B2C_PHASE_CLOCKS)
     if (d->d_clk.ensure(32 * 8)) return B2C_E_NOMEM;
-    CUDA_OK(cudaMemsetAsync(d->d_clk.p, 0, 32 * 8, st));
+    CUDA_OK(cudaMemsetAsync(d->d_clk.p, 0, 32 * 8, d->stream));
     BA.phase_clk = d->d_clk.as<u64>();
 #endif
+    return 0;
+}
 
-    struct Launch { int cls; size_t ord_off; int count; B2cLayout L; int slots; int per_sm; int threads; int v5; };
-    auto plan = [&](const std::vector<int>& utts, int cls, bool full, size_t ord_off) {
-        Launch ln;
-        ln.cls = cls;
-        ln.ord_off = ord_off;
-        ln.count = static_cast<int>(utts.size());
-        int tmax = 1;
-        u32 kmax = 1;
-        for (int u : utts) {
-            tmax = std::max(tmax, static_cast<int>(T[u]));
-            kmax = std::max(kmax, h_maxk[u]);
-        }
-        const u64 worst_m = static_cast<u64>(W_tab) * std::min<u32>(kmax, static_cast<u32>(V));
-        ln.v5 = (use_v5 && cls < kNumCaps) ? (use_lean ? 3 : v5_variant) : -1;
-        if (ln.v5 == 3) {
-            // lean variant: 32 slots, 128 candidates, no out-of-line tier (what does not fit is handed back)
-            ln.threads = 32;
-            ln.L = make_layout(32, V, tmax, full, smem_budget, 128, 0, 1);
-            ln.L.smem_bytes = static_cast<u32>(kV5Smem[3][V <= B2C_FAST_LT ? 1 : 0]);
-            ln.per_sm = kV5Occ[3];
-        } else if (ln.v5 >= 0) {
-            // beam tables of capacity 128; the HBM tier always exists (frames with more tokens than the rings hold use it too)
-            const u32 cap5 = kV5Cap[ln.v5];
-            ln.threads = kV5Threads[ln.v5];
-            // backtrack arena: fixed node ids of the frame steps below 128 * T, the out-of-line step allocates above
-            ln.L = make_layout(128, V, tmax, full, smem_budget, cap5, std::max<u64>(worst_m, cap5 + 1), B2C_FAST_NW,
-                               128ull * static_cast<u64>(std::max(tmax, 1)));
-            ln.L.smem_bytes = static_cast<u32>(kV5Smem[ln.v5][V <= B2C_FAST_LT ? 1 : 0]);
-            ln.per_sm = kV5Occ[ln.v5];
-        } else {
-        ln.threads = cls < kNumCaps ? threads_of(cls) : 128;
-        if (cls < kNumCaps) {
-            ln.L = layout_of(cls, tmax, full, worst_m);
-        } else {
-            // general kernel: the largest shared-memory candidate tier that fits (frames beyond it work on the HBM tier at
-            // L2 latency) -- unless the launch has more utterances than SMs and the small tier keeps two CTAs per SM
-            auto general = [&](u32 cap_max) {
-                return make_layout(W_tab, V, tmax, full, smem_budget, 0, worst_m, B2C_MAXWARPS, static_cast<u64>(s_max_beams),
-                                   s_max_words + static_cast<u64>(s_max_beams), n_lm, B2C_NBUCKET_WIDE, cap_max);
-            };
-            ln.L = general(2048);
-            if (per_sm_of(ln.L.smem_bytes, 128) == 1 && ln.count > d->n_sm) {
-                const B2cLayout small = general(512);
-                if (per_sm_of(small.smem_bytes, 128) >= 2) ln.L = small;
-            }
-        }
-        // the general kernel with room for one CTA per SM only (wide beams): that CTA gets the whole register file --
-        // its phases are loops over hundreds to thousands of candidates, each a chain of dependent memory accesses
-        if (cls == kNumCaps && per_sm_of(ln.L.smem_bytes, 128) == 1) ln.threads = 256;
-        // beam tables that do not fit shared memory (beam_width in the thousands) live in HBM: every phase is a chain of L2
-        // round trips, and twice the threads at half the registers hide more of them (with the tables in shared memory,
-        // e.g. beam 500, the spills cost more than they hide)
-        if (cls == kNumCaps && ln.threads == 256 && !ln.L.beams_in_smem) ln.threads = 512;
-        ln.per_sm = per_sm_of(ln.L.smem_bytes, ln.threads);
-        }
-        ln.slots = std::min(ln.count, d->n_sm * ln.per_sm);
-        const u64 budget = 16ull << 30;            // keep the HBM workspace bounded
-        if (static_cast<u64>(ln.slots) * ln.L.gws_bytes > budget)
-            ln.slots = static_cast<int>(std::max<u64>(1, budget / ln.L.gws_bytes));
-        return ln;
-    };
-    std::vector<Launch> launches;
-    size_t ord_used = 0;
-    auto plan_launches = [&](bool with_stats) {
-        h_maxk = with_stats ? d->h_maxk.as<u32>() : nostat_maxk.data();
-        h_sumk = with_stats ? d->h_sumk.as<u32>() : nostat_sumk.data();
-        classify();
-        launches.clear();
-        ord_used = 0;
-        for (int c = 0; c <= kNumCaps; ++c) {
-            if (classes[c].empty()) continue;
-            launches.push_back(plan(classes[c], c, false, ord_used));
-            for (int u : classes[c]) h_ord[ord_used++] = u;
-        }
-    };
-    plan_launches(!(pipe_candidate || hinted));
-    if (hinted && !(launches.size() == 1 && launches[0].v5 == d->plain_v5 && static_cast<int>(launches[0].L.cap_s) == d->plain_cap &&
-                    launches[0].slots == std::min(launches[0].count, d->n_sm * launches[0].per_sm))) {
+// The launch plan, then the work list, the workspace and what the decoder keeps of the plan.  Without this call's
+// statistics (pipelined and hinted calls) the worst case (V tokens in a frame) sizes the workspace; the capacity class
+// comes from the hint (one token per frame "on average" keeps the statistics-based bound out of its way).
+static int plan_call(b2c_decoder* d, Call& c) {
+    const Geometry& g = c.g;
+    const int n = g.n_utts;
+    cudaStream_t st = d->stream;
+    const bool nostat = g.pipelined || c.hinted;
+    if (nostat) { c.nostat_maxk.assign(n, static_cast<u32>(g.V)); c.nostat_sumk.assign(c.T, c.T + n); }
+    c.maxk = nostat ? c.nostat_maxk.data() : d->h_maxk.as<u32>();
+    c.plan = make_plan(g, c.maxk, nostat ? c.nostat_sumk.data() : d->h_sumk.as<u32>(), *d, c.k);
+    const std::vector<Launch>& ls = c.plan.launches;
+    if (c.hinted && !(ls.size() == 1 && ls[0].v5 == d->plain_v5 && static_cast<int>(ls[0].L.cap_s) == d->plain_cap &&
+                      ls[0].slots == std::min(ls[0].count, d->n_sm * ls[0].per_sm))) {
         // not the plan the last statistics-based call ran -- or the worst-case workspace of a plan without statistics (V tokens
         // in a frame: large alphabets) would cost resident CTAs: wait for this call's statistics and plan from them
-        hinted = false;
-        d->hinted_refused = true;
+        c.hinted = false; d->hinted_refused = true;
         CUDA_OK(cudaStreamSynchronize(st));
-        hp_mark(1);
-        plan_launches(true);
+        c.hp.mark(1);
+        c.maxk = d->h_maxk.as<u32>();
+        c.plan = make_plan(g, c.maxk, d->h_sumk.as<u32>(), *d, c.k);
     }
-    d->tm.hinted = hinted ? 1 : 0;
+    d->tm.hinted = c.hinted ? 1 : 0;
+    u32* h_next = reinterpret_cast<u32*>(c.hm + c.meta.next);
     for (size_t i = 0; i < 16; ++i) h_next[i] = 0;
-    CUDA_OK(cudaMemcpyAsync(d_ord, h_ord, 4 * ord_used, cudaMemcpyHostToDevice, st));
-    CUDA_OK(cudaMemcpyAsync(d_next, h_next, 64, cudaMemcpyHostToDevice, st));
-    // the classes run CONCURRENTLY (one stream each, forked from / joined to the decoder's stream):
-    // each launch's makespan is about one utterance's latency, serialising them would multiply it
+    std::copy(c.plan.ord.begin(), c.plan.ord.end(), c.h_ord());
+    CUDA_OK(cudaMemcpyAsync(c.d_ord(), c.h_ord(), 4 * c.plan.ord.size(), cudaMemcpyHostToDevice, st));
+    CUDA_OK(cudaMemcpyAsync(c.d_next(), h_next, 64, cudaMemcpyHostToDevice, st));
     u64 ws_need = 0;
-    std::vector<u64> ws_off;
-    for (const Launch& ln : launches) {
+    for (const Launch& ln : ls) {
         if (ln.L.smem_bytes > d->smem_optin) return fail(B2C_E_ARG, "beam_width too large for the shared-memory selection arrays");
-        ws_off.push_back(ws_need);
+        c.ws_off.push_back(ws_need);
         ws_need += static_cast<u64>(ln.slots) * ln.L.gws_bytes;
     }
     if (d->d_ws.ensure(ws_need)) return B2C_E_NOMEM;
-    // chunked launches need ONE launch of the latency-first kernel with every utterance resident
-    const bool can_chunk = launches.size() == 1 && launches[0].v5 >= 0 && launches[0].count <= launches[0].slots && !streaming;
-    if (pipe_candidate && !can_chunk) {
-        d->pipe_refused = true;                       // until the configuration (hint) changes
-        return B2C_E_RETRY_PLAIN;
+    if (c.plan.redo_plain) { d->pipe_refused = true; return B2C_E_RETRY_PLAIN; }   // until the configuration (hint) changes
+    // a plain call remembers its plan: pipelined and hinted calls of the configuration must plan the same
+    if (!g.pipelined && !c.hinted && ls.size() == 1 && c.plan.bounds.size() == 2) { d->plain_v5 = ls[0].v5; d->plain_cap = static_cast<int>(ls[0].L.cap_s); }
+    return 0;
+}
+
+// Pipelined and force-chunked calls: the plan's one latency-first launch runs gated (ONE launch behind the first chunk;
+// the streaming stage of the later chunks runs beside it on prep_stream and raises a flag per chunk) or as one launch
+// per chunk, state parked in HBM in between.  Pipelined calls copy the chunks on copy_stream and decide
+// probabilities-vs-logits at the end.
+static int enqueue_chunked(b2c_decoder* d, Call& c) {
+    const Launch& ln = c.plan.launches[0];
+    const std::vector<int>& bounds = c.plan.bounds;
+    const int n = c.g.n_utts, V = c.g.V, n_chunks = static_cast<int>(bounds.size()) - 1;
+    const bool gated = c.plan.gated, pipe = c.g.pipelined;
+    const size_t esz = c.g.esz;
+    cudaStream_t st = d->stream;
+    B2cBeamArgs& BA = c.BA;
+    const u64 stride = (kV5Save[ln.v5][V <= B2C_FAST_LT ? 1 : 0] + 16 + 255) & ~255ull;
+    if (d->d_state.ensure(stride * static_cast<u64>(ln.slots))) return B2C_E_NOMEM;
+    BA.L = ln.L; BA.n_utts = ln.count; BA.order = c.d_ord() + ln.ord_off; BA.next = c.d_next(); BA.gws = d->d_ws.as<u8>();
+    BA.state = d->d_state.as<u8>(); BA.state_stride = stride;
+    c.chunk_timing = pipe && n_chunks <= B2C_PIPE_CHUNKS;
+    cudaStream_t ps = gated ? static_cast<cudaStream_t>(d->prep_stream) : st;
+    if (gated) {
+        if (d->d_gate.ensure(64)) return B2C_E_NOMEM;
+        CUDA_OK(cudaMemsetAsync(d->d_gate.p, 0, 64, st));
+        CUDA_OK(cudaEventRecord(d->prep_ev[0], st));              // meta, memsets, hot table, LM states: uploaded
+        CUDA_OK(cudaStreamWaitEvent(ps, d->prep_ev[0], 0));
+        BA.gate = d->d_gate.as<u32>(); BA.gate_n = n_chunks;
+        for (int ch = 0; ch <= n_chunks; ++ch) BA.gate_bounds[ch] = bounds[ch];
     }
-    static const int force_chunks = std::getenv("B200CTC_FORCE_CHUNKS") ? std::atoi(std::getenv("B200CTC_FORCE_CHUNKS")) : 0;   // tests
-    // Chunk boundaries.  A chunked launch ends when its SLOWEST utterance has finished the chunk, so every boundary
-    // costs the spread of the per-chunk times.  Compute-bound calls (the copy is shorter than the decode) therefore use TWO chunks: a short first one whose
-    // decode covers the copy of the rest; copy-bound calls (large alphabets) use equal chunks.
-    std::vector<int> bounds{0, std::max(T_max, 0)};
-    // GATED launch (preferred for pipelined calls): ONE beam launch that starts after the first chunk and waits, on the
-    // device, for the flag of each later chunk -- no launch boundary, so no chunk pays for its slowest utterance.  The
-    // streaming stage of the later chunks runs CONCURRENTLY with the beam kernel on another stream, which needs free SM
-    // resources: only taken when the beam kernel leaves at least n_sm/8 CTA slots empty; a CTA that waits longer than
-    // ~40 ms gives up with B2C_ERR_GATE and the call is redone as a plain call.
-    // Which form of pipelining:
-    //   compute-bound calls (copy < 0.6 x decode, e.g. C2) -> the gated launch; chunked launches gain nothing there -- a
-    //     chunked launch ends when its slowest utterance has finished the chunk, so every boundary costs the spread of
-    //     the per-chunk times;
-    //   copy-bound calls (e.g. the C4 shape) -> chunked launches, equal chunks (the gated form is slower there: the
-    //     streaming stage of a 1 GB batch crawls on the SM slots the beam kernel leaves free).
-    // The plan of a pipelined call comes from the hint alone; it must be the plan the previous plain call of this
-    // configuration ran (another kernel variant would change the speed, not the result: diffuse batches decode 35 % slower
-    // on the latency-first kernel the hint-only plan picks than on the capacity-class kernel their statistics pick).
-    const double copy_ms_est = static_cast<double>(total_frames) * V * esz / 50.0e6;            // ~50 GB/s pinned H2D
-    const double pipe_r = copy_ms_est / std::max(d->last_device_ms > 0 ? d->last_device_ms : copy_ms_est, 1e-3);
-    const bool pipe_all = std::getenv("B200CTC_PIPELINE_ALL") != nullptr;
-    const bool gated = pipe_candidate && can_chunk && std::getenv("B200CTC_NO_GATE") == nullptr && (pipe_r < 0.6 || pipe_all) &&
-                       launches[0].count + d->n_sm / 8 <= d->n_sm * launches[0].per_sm;
-    if (pipe_candidate) {
-        const double r = pipe_r;
-        const bool same_plan = launches[0].v5 == d->plain_v5 && static_cast<int>(launches[0].L.cap_s) == d->plain_cap;
-        if ((!gated && r < 0.6 && !pipe_all) || (!same_plan && !pipe_all)) {
-            d->pipe_refused = true;
-            return B2C_E_RETRY_PLAIN;
+    if (pipe) {
+        // every chunk's copy is queued at once on the copy stream; the compute stream waits chunk by chunk
+        const size_t pitch = static_cast<size_t>(c.g.T_max) * V * esz;
+        for (int ch = 0; ch < n_chunks; ++ch) {
+            const int t0 = bounds[ch], t1 = bounds[ch + 1];
+            CUDA_OK(cudaMemcpy2DAsync(d->d_logits.as<char>() + static_cast<size_t>(t0) * V * esz, pitch,
+                                      static_cast<const char*>(c.logits[0]) + static_cast<size_t>(t0) * V * esz, pitch,
+                                      static_cast<size_t>(t1 - t0) * V * esz, static_cast<size_t>(n), cudaMemcpyHostToDevice, d->copy_stream));
+            CUDA_OK(cudaEventRecord(d->copied[ch % B2C_PIPE_CHUNKS], d->copy_stream));
+            d->tm.h2d_bytes += static_cast<long long>(t1 - t0) * V * static_cast<long long>(esz) * n;
         }
-        bounds.clear();
-        bounds.push_back(0);
-        if (!gated && r < 0.6) {
-            int f = static_cast<int>(1.15 * T_max * r / (1.0 + r));
-            f = std::max(2 * B2C_TILE_ROWS, ((f + B2C_TILE_ROWS - 1) / B2C_TILE_ROWS) * B2C_TILE_ROWS);
-            if (f < T_max) bounds.push_back(f);
-        } else {
-            for (int c = 1; c < B2C_PIPE_CHUNKS; ++c) if (c * chunk_len < T_max) bounds.push_back(c * chunk_len);
-        }
-        bounds.push_back(T_max);
-    } else if (can_chunk && force_chunks > 1 && T_max >= 2) {
-        const int nc = std::min(force_chunks, T_max), cl = (T_max + nc - 1) / nc;
-        bounds.clear();
-        for (int t0 = 0; t0 < T_max; t0 += cl) bounds.push_back(t0);
-        bounds.push_back(T_max);
     }
-    const int n_chunks = static_cast<int>(bounds.size()) - 1;
-    bool chunk_timing = false, gated_call = false;
-    if (n_chunks > 1) {
-        const Launch& ln = launches[0];
-        const u64 stride = (kV5Save[ln.v5][V <= B2C_FAST_LT ? 1 : 0] + 16 + 255) & ~255ull;
-        if (d->d_state.ensure(stride * static_cast<u64>(ln.slots))) return B2C_E_NOMEM;
-        BA.L = ln.L;
-        BA.n_utts = ln.count;
-        BA.order = d_ord + ln.ord_off;
-        BA.next = d_next;
-        BA.gws = d->d_ws.as<u8>();
-        BA.state = d->d_state.as<u8>();
-        BA.state_stride = stride;
-        chunk_timing = pipe_candidate && n_chunks <= B2C_PIPE_CHUNKS;
-        cudaStream_t ps = gated ? d->prep_stream : st;
+    if (!gated) CUDA_OK(cudaEventRecord(d->ev[5], st));
+#ifdef B2C_HOSTSIM
+    // hostsim runs a launch to completion at once: the gated launch goes behind the last chunk -- or, to test the give-up
+    // path (the later chunks "never arrive"), right behind the first one
+    const int beam_after = c.k.gate_early ? 0 : n_chunks - 1;
+#else
+    const int beam_after = 0;
+#endif
+    for (int ch = 0; ch < n_chunks; ++ch) {
+        const int t0 = bounds[ch], t1 = bounds[ch + 1];
+        if (pipe) {
+            CUDA_OK(cudaStreamWaitEvent(ps, d->copied[ch % B2C_PIPE_CHUNKS], 0));
+            if (c.chunk_timing) CUDA_OK(cudaEventRecord(d->chunk_ev[3 * ch], ps));
+            B2cPrepArgs PC = c.PA;
+            PC.mode = 0;
+            PC.tile_lo = t0 / B2C_TILE_ROWS; PC.tile_hi = (t1 + B2C_TILE_ROWS - 1) / B2C_TILE_ROWS;
+            PC.run_lo = t0 / B2C_RUN; PC.run_hi = (t1 + B2C_RUN - 1) / B2C_RUN;
+            B2C_TRY(launch_tokens(d, PC, c.f64, ps));
+            if (c.chunk_timing) CUDA_OK(cudaEventRecord(d->chunk_ev[3 * ch + 1], ps));
+        }
         if (gated) {
-            if (d->d_gate.ensure(64)) return B2C_E_NOMEM;
-            CUDA_OK(cudaMemsetAsync(d->d_gate.p, 0, 64, st));
-            CUDA_OK(cudaEventRecord(d->prep_ev[0], st));              // meta, memsets, hot table, LM states: uploaded
-            CUDA_OK(cudaStreamWaitEvent(ps, d->prep_ev[0], 0));
-            BA.gate = d->d_gate.as<u32>();
-            BA.gate_n = n_chunks;
-            for (int c = 0; c <= n_chunks; ++c) BA.gate_bounds[c] = bounds[c];
+            CUDA_OK(cudaMemsetAsync(d->d_gate.as<u32>() + ch, 1, 4, ps));       // chunk ch's token lists are in HBM
+            if (ch == beam_after) {
+                // the beam kernel: ONE launch, behind the first chunk only
+                CUDA_OK(cudaEventRecord(d->prep_ev[1], ps));
+                CUDA_OK(cudaStreamWaitEvent(st, d->prep_ev[1], 0));
+                CUDA_OK(cudaEventRecord(d->ev[5], st));
+                BA.chunk_t0 = 0; BA.chunk_t1 = 0;
+                B2C_TRY(launch_beam(d, BA, ln, st, true));
+            }
+            continue;
         }
-        if (pipe_candidate) {
-            // every chunk's copy is queued at once on the copy stream; the compute stream waits chunk by chunk
-            const size_t pitch = static_cast<size_t>(T_max) * V * esz;
-            for (int c = 0; c < n_chunks; ++c) {
-                const int t0 = bounds[c], t1 = bounds[c + 1];
-                CUDA_OK(cudaMemcpy2DAsync(d->d_logits.as<char>() + static_cast<size_t>(t0) * V * esz, pitch,
-                                          static_cast<const char*>(logits[0]) + static_cast<size_t>(t0) * V * esz, pitch,
-                                          static_cast<size_t>(t1 - t0) * V * esz, static_cast<size_t>(n_utts), cudaMemcpyHostToDevice, d->copy_stream));
-                CUDA_OK(cudaEventRecord(d->copied[c % B2C_PIPE_CHUNKS], d->copy_stream));
-                d->tm.h2d_bytes += static_cast<long long>(t1 - t0) * V * static_cast<long long>(esz) * n_utts;
-            }
-        }
-        if (!gated) CUDA_OK(cudaEventRecord(d->ev[5], st));
-        for (int c = 0; c < n_chunks; ++c) {
-            const int t0 = bounds[c], t1 = bounds[c + 1];
-            if (pipe_candidate) {
-                CUDA_OK(cudaStreamWaitEvent(ps, d->copied[c % B2C_PIPE_CHUNKS], 0));
-                if (chunk_timing) CUDA_OK(cudaEventRecord(d->chunk_ev[3 * c], ps));
-                B2cPrepArgs PC = PA;
-                PC.mode = 0;
-                PC.tile_lo = t0 / B2C_TILE_ROWS;
-                PC.tile_hi = (t1 + B2C_TILE_ROWS - 1) / B2C_TILE_ROWS;
-                PC.run_lo = t0 / B2C_RUN;
-                PC.run_hi = (t1 + B2C_RUN - 1) / B2C_RUN;
-                const u64 run_items = static_cast<u64>(n_utts) * static_cast<u64>(PC.run_hi - PC.run_lo);
-                const int grid_runs = static_cast<int>(std::max<u64>(1, std::min<u64>((run_items + B2C_PREP_WARPS - 1) / B2C_PREP_WARPS, static_cast<u64>(grid_tok))));
-#ifdef B2C_HOSTSIM
-                {
-                    std::unique_ptr<B2cPrepShared> sh(new B2cPrepShared());
-                    for (int b = 0; b < grid_runs; ++b) {
-                        if (dtype == B2C_DTYPE_F32) b2c_tokens_block<float>(PC, b, grid_runs, sh.get());
-                        else b2c_tokens_block<double>(PC, b, grid_runs, sh.get());
-                    }
-                }
-#else
-                if (dtype == B2C_DTYPE_F32 && V <= 32) {
-                    const u64 items = static_cast<u64>(n_utts) * static_cast<u64>(PC.tile_hi - PC.tile_lo);
-                    const int grid = static_cast<int>(std::max<u64>(1, std::min<u64>((items + B2C_TILE_WARPS - 1) / B2C_TILE_WARPS, static_cast<u64>(d->n_sm) * 8)));
-                    b2c_tokens_tile_kernel<<<grid, B2C_TILE_WARPS * 32, 0, ps>>>(PC);
-                } else if (dtype == B2C_DTYPE_F32) {
-                    b2c_tokens_kernel<float><<<grid_runs, B2C_PREP_THREADS, 0, ps>>>(PC);
-                } else {
-                    b2c_tokens_kernel<double><<<grid_runs, B2C_PREP_THREADS, 0, ps>>>(PC);
-                }
-                CUDA_OK(cudaGetLastError());
-#endif
-                d->tm.launches += 1;
-                if (chunk_timing) CUDA_OK(cudaEventRecord(d->chunk_ev[3 * c + 1], ps));
-            }
-            if (gated) {
-                CUDA_OK(cudaMemsetAsync(d->d_gate.as<u32>() + c, 1, 4, ps));       // chunk c's token lists are in HBM
-#ifdef B2C_HOSTSIM
-                // hostsim runs a launch to completion at once: after the last chunk -- or, to test the give-up path
-                // (the later chunks "never arrive"), right after the first one
-                if (c == (std::getenv("B200CTC_HOSTSIM_GATE_EARLY") ? 0 : n_chunks - 1)) {
-#else
-                if (c == 0) {
-#endif
-                    // the beam kernel: ONE launch, behind the first chunk only
-                    CUDA_OK(cudaEventRecord(d->prep_ev[1], ps));
-                    CUDA_OK(cudaStreamWaitEvent(st, d->prep_ev[1], 0));
-                    CUDA_OK(cudaEventRecord(d->ev[5], st));
-                    BA.chunk_t0 = 0;
-                    BA.chunk_t1 = 0;
-                    rc = launch_beam(d, BA, ln.slots, true, ln.per_sm, ln.threads, st, ln.v5);
-                    if (rc) return rc;
-                    d->tm.launches += 1;
-                }
-                continue;
-            }
-            BA.chunk_t0 = t0;
-            BA.chunk_t1 = t1;
-            BA.chunk_last = c == n_chunks - 1 ? 1 : 0;
-            rc = launch_beam(d, BA, ln.slots, true, ln.per_sm, ln.threads, st, ln.v5);
-            if (rc) return rc;
-            d->tm.launches += 1;
-            if (chunk_timing) CUDA_OK(cudaEventRecord(d->chunk_ev[3 * c + 2], st));
-        }
-        BA.chunk_t1 = 0;
-        BA.gate = nullptr;
-        if (pipe_candidate) {
-            // probabilities or logits: decided now that every row has been seen; a probability utterance voids the call
-#ifdef B2C_HOSTSIM
-            {
-                std::unique_ptr<B2cDecideShared> dsh(new B2cDecideShared());
-                for (int u = 0; u < n_utts; ++u) {
-                    if (dtype == B2C_DTYPE_F32) b2c_decide_block<float>(PA, u, dsh.get());
-                    else b2c_decide_block<double>(PA, u, dsh.get());
-                }
-            }
-#else
-            if (dtype == B2C_DTYPE_F32) b2c_decide_kernel<float><<<n_utts, 128, 0, ps>>>(PA);
-            else b2c_decide_kernel<double><<<n_utts, 128, 0, ps>>>(PA);
-            CUDA_OK(cudaGetLastError());
-#endif
-            d->tm.launches += 1;
-            if (gated) {
-                CUDA_OK(cudaEventRecord(d->prep_ev[2], ps));
-                CUDA_OK(cudaStreamWaitEvent(st, d->prep_ev[2], 0));
-            }
-            CUDA_OK(cudaMemcpyAsync(d->h_maxk.p, d->d_approx.as<double>() + 2 * n_utts, 4, cudaMemcpyDeviceToHost, st));
-        }
-        gated_call = gated;
-        d->tm.cap_candidates = static_cast<int>(ln.L.cap_s);
-        d->tm.cta_threads = ln.threads;
-        d->tm.cta_slots = ln.slots;
-        d->tm.kernel_variant = 2;
+        BA.chunk_t0 = t0; BA.chunk_t1 = t1; BA.chunk_last = ch == n_chunks - 1 ? 1 : 0;
+        B2C_TRY(launch_beam(d, BA, ln, st, true));
+        if (c.chunk_timing) CUDA_OK(cudaEventRecord(d->chunk_ev[3 * ch + 2], st));
     }
-    if (n_chunks == 1) CUDA_OK(cudaEventRecord(d->ev[5], st));
+    BA.chunk_t1 = 0; BA.gate = nullptr;
+    if (pipe) {
+        // probabilities or logits: decided now that every row has been seen; a probability utterance voids the call
+        B2C_TRY(launch_decide(d, c.PA, c.f64, ps));
+        if (gated) {
+            CUDA_OK(cudaEventRecord(d->prep_ev[2], ps));
+            CUDA_OK(cudaStreamWaitEvent(st, d->prep_ev[2], 0));
+        }
+        CUDA_OK(cudaMemcpyAsync(d->h_maxk.p, d->d_approx.as<double>() + 2 * n, 4, cudaMemcpyDeviceToHost, st));
+    }
+    c.gated_call = gated;
+    return 0;
+}
+
+// the launches of an unchunked call; the classes run CONCURRENTLY (one stream each, forked from / joined to the decoder's
+// stream): each launch's makespan is about one utterance's latency, serialising them would multiply it
+static int enqueue_plain(b2c_decoder* d, Call& c) {
+    const std::vector<Launch>& ls = c.plan.launches;
+    const bool chunked = c.plan.bounds.size() > 2;
+    cudaStream_t st = d->stream;
+    if (!chunked) CUDA_OK(cudaEventRecord(d->ev[5], st));
     CUDA_OK(cudaEventRecord(d->fork_ev, st));
-    int qi = 0;
-    for (const Launch& ln : launches) {
-        if (n_chunks > 1) break;
-        cudaStream_t cs = launches.size() > 1 ? d->cls_stream[ln.cls < kNumCaps ? 0 : 1] : st;
+    for (size_t qi = 0; qi < ls.size() && !chunked; ++qi) {
+        const Launch& ln = ls[qi];
+        const int lane = ln.cls < kNumCaps ? 0 : 1;           // fast class, general kernel
+        cudaStream_t cs = ls.size() > 1 ? static_cast<cudaStream_t>(d->cls_stream[lane]) : st;
         if (cs != st) CUDA_OK(cudaStreamWaitEvent(cs, d->fork_ev, 0));
-        BA.L = ln.L;
-        BA.n_utts = ln.count;
-        BA.order = d_ord + ln.ord_off;
-        BA.next = d_next + qi;
-        BA.gws = d->d_ws.as<u8>() + ws_off[qi];
-        ++qi;
-        rc = launch_beam(d, BA, ln.slots, ln.cls < kNumCaps, ln.per_sm, ln.threads, cs, ln.v5);
-        if (rc) return rc;
-        d->tm.launches += 1;
-        if (ln.cls < kNumCaps || launches.size() == 1) {
-            d->tm.cap_candidates = static_cast<int>(ln.L.cap_s);
-            d->tm.cta_threads = ln.threads;
-            d->tm.cta_slots = ln.slots;
-            d->tm.kernel_variant = ln.v5 >= 0 ? 2 : (ln.cls < kNumCaps ? 1 : 0);
-            if (!pipe_candidate && !hinted && launches.size() == 1) { d->plain_v5 = ln.v5; d->plain_cap = static_cast<int>(ln.L.cap_s); }
-        }
-        if (cs != st) {
-            CUDA_OK(cudaEventRecord(d->cls_done[ln.cls < kNumCaps ? 0 : 1], cs));
-            CUDA_OK(cudaStreamWaitEvent(st, d->cls_done[ln.cls < kNumCaps ? 0 : 1], 0));
-        }
+        c.BA.L = ln.L; c.BA.n_utts = ln.count; c.BA.order = c.d_ord() + ln.ord_off;
+        c.BA.next = c.d_next() + qi; c.BA.gws = d->d_ws.as<u8>() + c.ws_off[qi];
+        B2C_TRY(launch_beam(d, c.BA, ln, cs, ln.cls < kNumCaps || ls.size() == 1));
+        if (cs != st) CUDA_OK(cudaEventRecord(d->cls_done[lane], cs));
+        if (cs != st) CUDA_OK(cudaStreamWaitEvent(st, d->cls_done[lane], 0));
     }
     CUDA_OK(cudaEventRecord(d->ev[3], st));
+    return 0;
+}
 
-    // ---- device -> host -------------------------------------------------------------------
-    CUDA_OK(cudaMemcpyAsync(d->h_out_small.p, d->d_out_small.p, small_bytes, cudaMemcpyDeviceToHost, st));
-    CUDA_OK(cudaMemcpyAsync(d->h_out_toks.p, d->d_out_toks.p, tok_bytes, cudaMemcpyDeviceToHost, st));
-    const bool text_only = opts->text_only != 0 && !streaming;
-    if (!text_only) CUDA_OK(cudaMemcpyAsync(d->h_out_frames.p, d->d_out_frames.p, frm_bytes, cudaMemcpyDeviceToHost, st));
+static int read_outputs(b2c_decoder* d, const Call& c, bool frames) {
+    CUDA_OK(cudaMemcpyAsync(d->h_out_small.p, d->d_out_small.p, c.out.bytes, cudaMemcpyDeviceToHost, d->stream));
+    CUDA_OK(cudaMemcpyAsync(d->h_out_toks.p, d->d_out_toks.p, c.tok_bytes, cudaMemcpyDeviceToHost, d->stream));
+    if (frames) CUDA_OK(cudaMemcpyAsync(d->h_out_frames.p, d->d_out_frames.p, c.frm_bytes, cudaMemcpyDeviceToHost, d->stream));
+    return 0;
+}
+
+// device -> host, then the hint the next call of this configuration plans from
+static int read_back(b2c_decoder* d, Call& c) {
+    const int n = c.g.n_utts;
+    cudaStream_t st = d->stream;
+    B2C_TRY(read_outputs(d, c, !c.text_only));
     if (d->h_mstats.ensure(64)) return B2C_E_NOMEM;
     CUDA_OK(cudaMemcpyAsync(d->h_mstats.p, d->d_mstats.p, 64, cudaMemcpyDeviceToHost, st));
     // selected-token totals (b2c_timings_t.tokens); a plain call already copied them for the launch plan
-    if (pipe_candidate) CUDA_OK(cudaMemcpyAsync(d->h_sumk.p, d->d_sumk.p, 4ull * n_utts, cudaMemcpyDeviceToHost, st));
+    if (c.g.pipelined) CUDA_OK(cudaMemcpyAsync(d->h_sumk.p, d->d_sumk.p, 4ull * n, cudaMemcpyDeviceToHost, st));
     CUDA_OK(cudaEventRecord(d->ev[4], st));
-    hp_mark(2);                                   // launch planning + enqueue of the beam kernel and D2H
+    c.hp.mark(2);                                 // launch planning + enqueue of the beam kernel and D2H
     CUDA_OK(cudaStreamSynchronize(st));
-    hp_mark(3);                                   // wait: beam kernel + D2H
-    if (pipe_candidate && d->h_maxk.as<u32>()[0] != 0) return B2C_E_RETRY_PLAIN;   // some utterance holds probabilities
-    if (gated_call) {
-        const int* hst = reinterpret_cast<const int*>(d->h_out_small.as<u8>() + off_st);
-        for (int i = 0; i < n_utts; ++i)
-            if (hst[i] & B2C_ERR_GATE) {           // the streaming stage of a later chunk never got to run beside the beam kernel
-                d->pipe_refused = true;
-                return B2C_E_RETRY_PLAIN;
-            }
+    c.hp.mark(3);                                 // wait: beam kernel + D2H
+    if (c.g.pipelined && d->h_maxk.as<u32>()[0] != 0) return B2C_E_RETRY_PLAIN;   // some utterance holds probabilities
+    if (c.gated_call) {
+        const int* status = c.out.at(d->h_out_small.as<u8>()).status;
+        // the streaming stage of a later chunk never got to run beside the beam kernel
+        for (int i = 0; i < n; ++i) if (status[i] & B2C_ERR_GATE) { d->pipe_refused = true; return B2C_E_RETRY_PLAIN; }
     }
-    d->tm.d2h_bytes += static_cast<long long>(small_bytes + tok_bytes + (text_only ? 0 : frm_bytes) + 8ull * n_utts + 32);
-    {
-        const u32* ms = d->h_mstats.as<u32>();
-        d->hint_valid = true;
-        d->hint_beam = opts->beam_width;
-        d->hint_lm = P.lm.order > 0 ? 1 : 0;
-        d->hint_hot = P.n_hot > 0 ? 1 : 0;
-        d->hint_prune = P.prune_history;
-        for (int q = 0; q < 6; ++q) d->hint_over[q] = ms[q];
-        d->hint_frames = ms[6];
-        for (int q = 0; q < 7; ++q) d->tm.cand_hist[q] = ms[q];
-        d->tm.inplace_frames = ms[7];
-        d->tm.sorted_frames = ms[8];
-        d->hint_wide_utts = ms[9];
-        d->hint_utts = ms[10];
-        d->tm.oversize_frames = 0;
-        for (int q = 0; q < 6; ++q)
-            if (static_cast<int>(128u << q) == d->tm.cap_candidates) d->tm.oversize_frames = ms[q];
-    }
+    d->tm.d2h_bytes += static_cast<long long>(c.out.bytes + c.tok_bytes + (c.text_only ? 0 : c.frm_bytes) + 8ull * n + 32);
+    const u32* ms = d->h_mstats.as<u32>();
+    d->hint_valid = true;
+    d->hint_beam = c.opts->beam_width; d->hint_lm = c.P.lm.order > 0 ? 1 : 0; d->hint_hot = c.P.n_hot > 0 ? 1 : 0; d->hint_prune = c.P.prune_history;
+    for (int q = 0; q < 6; ++q) d->hint_over[q] = ms[q];
+    d->hint_frames = ms[6];
+    for (int q = 0; q < 7; ++q) d->tm.cand_hist[q] = ms[q];
+    d->tm.inplace_frames = ms[7]; d->tm.sorted_frames = ms[8];
+    d->hint_wide_utts = ms[9]; d->hint_utts = ms[10];
+    d->tm.oversize_frames = 0;
+    for (int q = 0; q < 6; ++q)
+        if (static_cast<int>(128u << q) == d->tm.cap_candidates) d->tm.oversize_frames = ms[q];
+    return 0;
+}
 
-    u8* hs = d->h_out_small.as<u8>();
-    int* h_status = reinterpret_cast<int*>(hs + off_st);
+// retry passes: (1) utterances the lean variant handed back -> a full latency-first variant; (2) utterances whose
+// arenas overflowed -> the general kernel with worst-case arenas
+static int retry_failed(b2c_decoder* d, Call& c) {
+    const int n = c.g.n_utts;
+    cudaStream_t st = d->stream;
+    const int* status = c.out.at(d->h_out_small.as<u8>()).status;
     std::vector<int> failed;
-    for (int i = 0; i < n_utts; ++i) if (h_status[i] != B2C_OK) failed.push_back(i);
-    if (use_lean && 10 * failed.size() > static_cast<size_t>(n_utts)) d->lean_bad = true;     // not worth it for this configuration
-    // retry passes: (1) utterances the lean variant handed back -> a full latency-first variant; (2) utterances whose
-    // arenas overflowed -> the general kernel with worst-case arenas
+    for (int i = 0; i < n; ++i) if (status[i] != B2C_OK) failed.push_back(i);
+    if (c.plan.use_lean && 10 * failed.size() > static_cast<size_t>(n)) d->lean_bad = true;     // not worth it for this configuration
     for (int pass = 0; pass < 2 && !failed.empty(); ++pass) {
-        bool only_slots = use_lean && pass == 0;
-        for (int i : failed) only_slots = only_slots && h_status[i] == B2C_ERR_SLOTS;
+        bool only_slots = c.plan.use_lean && pass == 0;
+        for (int i : failed) only_slots = only_slots && status[i] == B2C_ERR_SLOTS;
         if (pass == 0 && !only_slots) continue;
-        Launch ln;
+        int cls = kNumCaps;
         if (only_slots) {
-            use_lean = false;
-            int fast_cls = 0;
-            for (const Launch& l0 : launches) if (l0.v5 >= 0) fast_cls = l0.cls;
-            ln = plan(failed, fast_cls, false, static_cast<size_t>(n_utts));
-        } else {
-            ln = plan(failed, kNumCaps, true, static_cast<size_t>(n_utts));
+            c.plan.use_lean = false;
+            cls = 0;
+            for (const Launch& l0 : c.plan.launches) if (l0.v5 >= 0) cls = l0.cls;
         }
+        const Launch ln = plan_launch(c.g, c.maxk, c.plan, d->n_sm, failed, cls, !only_slots, static_cast<size_t>(n));
         if (ln.L.smem_bytes > d->smem_optin) return fail(B2C_E_ARG, "beam_width too large for the shared-memory selection arrays");
         if (d->d_ws.ensure(static_cast<u64>(ln.slots) * ln.L.gws_bytes)) return B2C_E_NOMEM;
-        for (size_t i = 0; i < failed.size(); ++i) h_ord[n_utts + i] = failed[i];
-        CUDA_OK(cudaMemcpyAsync(d_ord + n_utts, h_ord + n_utts, 4 * failed.size(), cudaMemcpyHostToDevice, st));
-        CUDA_OK(cudaMemsetAsync(d_next + 15, 0, 4, st));
-        BA.L = ln.L;
-        BA.n_utts = ln.count;
-        BA.order = d_ord + n_utts;
-        BA.next = d_next + 15;
-        BA.gws = d->d_ws.as<u8>();
-        BA.chunk_t1 = 0;
-        rc = launch_beam(d, BA, ln.slots, ln.cls < kNumCaps, ln.per_sm, ln.threads, st, ln.v5);
-        if (rc) return rc;
-        d->tm.launches += 1;
-        CUDA_OK(cudaMemcpyAsync(d->h_out_small.p, d->d_out_small.p, small_bytes, cudaMemcpyDeviceToHost, st));
-        CUDA_OK(cudaMemcpyAsync(d->h_out_toks.p, d->d_out_toks.p, tok_bytes, cudaMemcpyDeviceToHost, st));
-        CUDA_OK(cudaMemcpyAsync(d->h_out_frames.p, d->d_out_frames.p, frm_bytes, cudaMemcpyDeviceToHost, st));
+        int* h_ord = c.h_ord();
+        for (size_t i = 0; i < failed.size(); ++i) h_ord[n + i] = failed[i];
+        CUDA_OK(cudaMemcpyAsync(c.d_ord() + n, h_ord + n, 4 * failed.size(), cudaMemcpyHostToDevice, st));
+        CUDA_OK(cudaMemsetAsync(c.d_next() + 15, 0, 4, st));
+        c.BA.L = ln.L; c.BA.n_utts = ln.count; c.BA.order = c.d_ord() + n; c.BA.next = c.d_next() + 15; c.BA.gws = d->d_ws.as<u8>();
+        c.BA.chunk_t1 = 0;
+        B2C_TRY(launch_beam(d, c.BA, ln, st, false));
+        B2C_TRY(read_outputs(d, c, true));
         CUDA_OK(cudaStreamSynchronize(st));
         std::vector<int> still;
-        for (int i : failed) if (h_status[i] != B2C_OK) still.push_back(i);
+        for (int i : failed) if (status[i] != B2C_OK) still.push_back(i);
         failed.swap(still);
     }
     for (int i : failed)
-        return fail(B2C_E_INTERNAL, "beam kernel workspace overflow (status " + std::to_string(h_status[i]) + ")");
+        return fail(B2C_E_INTERNAL, "beam kernel workspace overflow (status " + std::to_string(status[i]) + ")");
+    return 0;
+}
+
+static int record_timings(b2c_decoder* d, const Call& c) {
 #if defined(B2C_PHASE_CLOCKS)
     {
         u64 hc[32];
         CUDA_OK(cudaMemcpy(hc, d->d_clk.p, sizeof(hc), cudaMemcpyDeviceToHost));
         std::fprintf(stderr, "[b2c phase clocks, summed over CTAs, Mcycles]");
         for (int q = 0; q < 24; ++q) std::fprintf(stderr, " p%d=%.3f", q, hc[q] / 1e6);
-        std::fprintf(stderr, "  frames=%llu\n", static_cast<unsigned long long>(total_frames));
+        std::fprintf(stderr, "  frames=%llu\n", static_cast<unsigned long long>(c.g.total_frames));
     }
 #endif
+    const int n_chunks = static_cast<int>(c.plan.bounds.size()) - 1;
     float ms = 0.f;
-    if (chunk_timing) {        // pipelined: kernels of the chunks interleave with waits for the copies -- sum them up
+    if (c.chunk_timing) {        // pipelined: kernels of the chunks interleave with waits for the copies -- sum them up
         float mp = 0.f, mb = 0.f;
-        for (int c = 0; c < n_chunks; ++c) {
-            if (cudaEventElapsedTime(&ms, d->chunk_ev[3 * c], d->chunk_ev[3 * c + 1]) == cudaSuccess) mp += ms;
-            if (!gated_call && cudaEventElapsedTime(&ms, d->chunk_ev[3 * c + 1], d->chunk_ev[3 * c + 2]) == cudaSuccess) mb += ms;
+        for (int ch = 0; ch < n_chunks; ++ch) {
+            if (cudaEventElapsedTime(&ms, d->chunk_ev[3 * ch], d->chunk_ev[3 * ch + 1]) == cudaSuccess) mp += ms;
+            if (!c.gated_call && cudaEventElapsedTime(&ms, d->chunk_ev[3 * ch + 1], d->chunk_ev[3 * ch + 2]) == cudaSuccess) mb += ms;
         }
-        if (gated_call && cudaEventElapsedTime(&ms, d->ev[5], d->ev[3]) == cudaSuccess) mb = ms;     // one launch, waits included
-        d->tm.ms_prepare = mp;
-        d->tm.ms_beam = mb;
-        if (host_prof) {
+        if (c.gated_call && cudaEventElapsedTime(&ms, d->ev[5], d->ev[3]) == cudaSuccess) mb = ms;     // one launch, waits included
+        d->tm.ms_prepare = mp; d->tm.ms_beam = mb;
+        if (c.k.host_prof) {
             std::fprintf(stderr, "[b2c pipeline, ms after the call's first event]");
-            for (int c = 0; c < n_chunks; ++c) {
+            for (int ch = 0; ch < n_chunks; ++ch) {
                 float a0 = 0.f, a1 = 0.f, a2 = 0.f;
-                cudaEventElapsedTime(&a0, d->ev[0], d->chunk_ev[3 * c]);
-                cudaEventElapsedTime(&a1, d->ev[0], d->chunk_ev[3 * c + 1]);
-                if (!gated_call) cudaEventElapsedTime(&a2, d->ev[0], d->chunk_ev[3 * c + 2]);
-                std::fprintf(stderr, "  chunk %d: copied %.3f streamed %.3f decoded %.3f", c, a0, a1, a2);
+                cudaEventElapsedTime(&a0, d->ev[0], d->chunk_ev[3 * ch]);
+                cudaEventElapsedTime(&a1, d->ev[0], d->chunk_ev[3 * ch + 1]);
+                if (!c.gated_call) cudaEventElapsedTime(&a2, d->ev[0], d->chunk_ev[3 * ch + 2]);
+                std::fprintf(stderr, "  chunk %d: copied %.3f streamed %.3f decoded %.3f", ch, a0, a1, a2);
             }
             float a4 = 0.f;
             cudaEventElapsedTime(&a4, d->ev[0], d->ev[4]);
             std::fprintf(stderr, "  d2h done %.3f\n", a4);
         }
     } else {
-        if (!pipe_candidate && cudaEventElapsedTime(&ms, d->ev[1], d->ev[2]) == cudaSuccess) d->tm.ms_prepare = ms;
+        if (!c.g.pipelined && cudaEventElapsedTime(&ms, d->ev[1], d->ev[2]) == cudaSuccess) d->tm.ms_prepare = ms;
         if (cudaEventElapsedTime(&ms, d->ev[5], d->ev[3]) == cudaSuccess) d->tm.ms_beam = ms;
     }
     if (cudaEventElapsedTime(&ms, d->ev[0], d->ev[4]) == cudaSuccess) d->tm.ms_total = ms;
-    d->tm.frames = static_cast<long long>(total_frames);
+    d->tm.frames = static_cast<long long>(c.g.total_frames);
     d->last_device_ms = static_cast<double>(d->tm.ms_prepare) + static_cast<double>(d->tm.ms_beam);
     d->tm.tokens = 0;
-    for (int i = 0; i < n_utts; ++i) d->tm.tokens += static_cast<long long>(d->h_sumk.as<u32>()[i]);
-    d->last_T.assign(T, T + n_utts);
+    for (int i = 0; i < c.g.n_utts; ++i) d->tm.tokens += static_cast<long long>(d->h_sumk.as<u32>()[i]);
+    d->last_T.assign(c.T, c.T + c.g.n_utts);
+    return 0;
+}
 
-    // ---- assemble results -------------------------------------------------------------------
-    const int* h_nb = reinterpret_cast<const int*>(hs + off_nb);
-    const double* h_sc = reinterpret_cast<const double*>(hs + off_sc);
-    const int* h_nt = reinterpret_cast<const int*>(hs + off_nt);
-    const int* h_nw = reinterpret_cast<const int*>(hs + off_nw);
-    const B2cLmState* h_ls = reinterpret_cast<const B2cLmState*>(hs + off_ls);
-    const int* h_ax = streaming ? reinterpret_cast<const int*>(hs + off_ax) : nullptr;
-    const B2cLmState* h_lx = n_lm > 1 ? reinterpret_cast<const B2cLmState*>(hs + off_lx) : nullptr;
+static void assemble_range(const b2c_decoder* d, const Call& c, b2c_result* res, int u0, int u1) {
+    const OutViews h = c.out.at(d->h_out_small.as<u8>());
     const u32* h_toks = d->h_out_toks.as<u32>();
     const int* h_frames = d->h_out_frames.as<int>();
-    auto assemble_range = [&](int u0, int u1) {
-        for (int u = u0; u < u1; ++u) {
-            const int nb = h_nb[u];
-            res->utts[u].resize(nb);
-            const u64 base = static_cast<u64>(OB) * (frame_off[u] + static_cast<u64>(u));
-            const u64 stride = static_cast<u64>(T[u]) + 1;
-            for (int r = 0; r < nb; ++r) {
-                BeamRes& br = res->utts[u][r];
-                const u64 k = static_cast<u64>(u) * OB + r;
-                br.logit = h_sc[2 * k];
-                br.lm = h_sc[2 * k + 1];
-                br.st = h_ls[k];
-                if (h_lx) br.stx.assign(h_lx + k * (n_lm - 1), h_lx + (k + 1) * (n_lm - 1));
-                if (text_only) assemble_text(d, h_toks + base + r * stride, h_nt[k], br);
-                else assemble_beam(d, h_toks + base + r * stride, h_nt[k], h_frames + 2 * (base + r * stride), h_nw[k], br);
-                if (h_ax) {
-                    const u32* tk = h_toks + base + r * stride;
-                    br.raw.resize(static_cast<size_t>(h_nt[k]));
-                    for (int q = 0; q < h_nt[k]; ++q) br.raw[q] = tk[h_nt[k] - 1 - q];
-                    for (int q = 0; q < 4; ++q) br.aux[q] = h_ax[4 * k + q];
-                    {   // the chain as strings (the host replays it onto the input beam's text / partial word)
-                        std::string cur;
-                        br.s_boundary = false;
-                        for (const u32 v : br.raw) {
-                            const u32 tok = v & 0xFFFFu, kind = v >> 16;
-                            if (kind == B2C_CK_CONT) { cur += d->labels[tok]; continue; }
-                            if (!br.s_boundary) { br.s_first = cur; br.s_boundary = true; }
-                            else if (!cur.empty()) { if (!br.s_mid.empty()) br.s_mid += ' '; br.s_mid += cur; }
-                            cur = kind == B2C_CK_BPE ? d->clean[tok] : std::string();
-                        }
-                        if (br.s_boundary) br.s_last = cur; else br.s_first = cur;
+    const int OB = c.OB, n_lm = c.g.n_lm;
+    for (int u = u0; u < u1; ++u) {
+        const int nb = h.nbeams[u];
+        res->utts[u].resize(nb);
+        const u64 base = static_cast<u64>(OB) * (c.frame_off[u] + static_cast<u64>(u));
+        const u64 stride = static_cast<u64>(c.T[u]) + 1;
+        for (int r = 0; r < nb; ++r) {
+            BeamRes& br = res->utts[u][r];
+            const u64 k = static_cast<u64>(u) * OB + r;
+            br.logit = h.scores[2 * k];
+            br.lm = h.scores[2 * k + 1];
+            br.st = h.states[k];
+            if (h.states_x) br.stx.assign(h.states_x + k * (n_lm - 1), h.states_x + (k + 1) * (n_lm - 1));
+            if (c.text_only) assemble_text(d, h_toks + base + r * stride, h.ntok[k], br);
+            else assemble_beam(d, h_toks + base + r * stride, h.ntok[k], h_frames + 2 * (base + r * stride), h.nwords[k], br);
+            if (h.aux) {
+                const u32* tk = h_toks + base + r * stride;
+                br.raw.resize(static_cast<size_t>(h.ntok[k]));
+                for (int q = 0; q < h.ntok[k]; ++q) br.raw[q] = tk[h.ntok[k] - 1 - q];
+                for (int q = 0; q < 4; ++q) br.aux[q] = h.aux[4 * k + q];
+                {   // the chain as strings (the host replays it onto the input beam's text / partial word)
+                    std::string cur;
+                    br.s_boundary = false;
+                    for (const u32 v : br.raw) {
+                        const u32 tok = v & 0xFFFFu, kind = v >> 16;
+                        if (kind == B2C_CK_CONT) { cur += d->labels[tok]; continue; }
+                        if (!br.s_boundary) { br.s_first = cur; br.s_boundary = true; }
+                        else if (!cur.empty()) { if (!br.s_mid.empty()) br.s_mid += ' '; br.s_mid += cur; }
+                        cur = kind == B2C_CK_BPE ? d->clean[tok] : std::string();
                     }
-                    // assemble_beam truncated the frame list to the words it could name; keep all of them here
-                    br.frames.resize(static_cast<size_t>(h_nw[k]) * 2);
-                    const int* fr = h_frames + 2 * (base + r * stride);
-                    for (int w = 0; w < h_nw[k]; ++w) {
-                        br.frames[2 * w] = fr[2 * (h_nw[k] - 1 - w)];
-                        br.frames[2 * w + 1] = fr[2 * (h_nw[k] - 1 - w) + 1];
-                    }
+                    if (br.s_boundary) br.s_last = cur; else br.s_first = cur;
+                }
+                // assemble_beam truncated the frame list to the words it could name; keep all of them here
+                br.frames.resize(static_cast<size_t>(h.nwords[k]) * 2);
+                const int* fr = h_frames + 2 * (base + r * stride);
+                for (int w = 0; w < h.nwords[k]; ++w) {
+                    br.frames[2 * w] = fr[2 * (h.nwords[k] - 1 - w)];
+                    br.frames[2 * w + 1] = fr[2 * (h.nwords[k] - 1 - w) + 1];
                 }
             }
         }
-    };
-    {
-        // string building is independent per utterance: a few persistent host threads for large batches
-        const u64 work = (total_frames + static_cast<u64>(n_utts)) * static_cast<u64>(OB);
-        int n_thr = static_cast<int>(std::min<u64>(std::min<u64>(8, std::max(1u, std::thread::hardware_concurrency())), work / 32768));
-        n_thr = std::min(n_thr, n_utts);
-        if (n_thr <= 1) {
-            assemble_range(0, n_utts);
-        } else {
-            if (!d->pool) {
-                d->pool.reset(new HostPool());
-                d->pool->start(static_cast<int>(std::min<u64>(8, std::max(1u, std::thread::hardware_concurrency()))) - 1);
-            }
-            const int chunks = n_thr * 4;
-            const int per = (n_utts + chunks - 1) / chunks;
-            const std::function<void(int)> task = [&](int c) { assemble_range(std::min(n_utts, c * per), std::min(n_utts, (c + 1) * per)); };
-            d->pool->run(chunks, task);
-        }
     }
-    hp_mark(4);                                   // statistics read-back, result assembly
-    if (host_prof)
-        std::fprintf(stderr, "[b2c host ms] enqueue=%.3f wait_prepare=%.3f plan=%.3f wait_beam=%.3f assemble=%.3f\n", hp_ms[0],
-                     hp_ms[1], hp_ms[2], hp_ms[3], hp_ms[4]);
+}
+
+// string building is independent per utterance: a few persistent host threads for large batches
+static void assemble(b2c_decoder* d, const Call& c, b2c_result* res) {
+    const int n = c.g.n_utts;
+    res->n_models = c.g.n_lm;
+    res->streaming = c.g.streaming;
+    const u64 work = (c.g.total_frames + static_cast<u64>(n)) * static_cast<u64>(c.OB);
+    int n_thr = static_cast<int>(std::min<u64>(std::min<u64>(8, std::max(1u, std::thread::hardware_concurrency())), work / 32768));
+    n_thr = std::min(n_thr, n);
+    if (n_thr <= 1) return assemble_range(d, c, res, 0, n);
+    if (!d->pool) {
+        d->pool.reset(new HostPool());
+        d->pool->start(static_cast<int>(std::min<u64>(8, std::max(1u, std::thread::hardware_concurrency()))) - 1);
+    }
+    const int chunks = n_thr * 4, per = (n + chunks - 1) / chunks;
+    const std::function<void(int)> task = [&](int q) { assemble_range(d, c, res, std::min(n, q * per), std::min(n, (q + 1) * per)); };
+    d->pool->run(chunks, task);
+}
+
+static int decode_batch_locked(b2c_decoder_t* d, const void* const* logits, const int32_t* T, int n_utts, int dtype, int is_device,
+                               const b2c_decode_opts_t* opts, b2c_result_t** out, bool allow_pipe) {
+    if (dtype < B2C_DTYPE_F32 || dtype > B2C_DTYPE_BF16) return fail(B2C_E_ARG, "dtype must be one of B2C_DTYPE_F32 / F64 / F16 / BF16");
+    Call c(d, logits, T, n_utts, dtype, is_device, opts, allow_pipe);
+    d->last_T.clear();
+    if (opts->beam_width < 1) return fail(B2C_E_ARG, "beam_width must be >= 1");
+    if (opts->beam_width > 65535) return fail(B2C_E_ARG, "beam_width above 65535 is not supported");
+    std::unique_ptr<b2c_result> res(new b2c_result());
+    res->utts.resize(n_utts); res->has_lm = d->lm != nullptr;
+    if (n_utts == 0) { *out = res.release(); return 0; }
+    CUDA_OK(cudaSetDevice(d->device));
+    std::memset(&d->tm, 0, sizeof(d->tm));
+    B2C_TRY(set_geometry(c));
+    B2C_TRY(flatten_stream_states(d, c));
+    B2C_TRY(make_params(d, c));
+    B2C_TRY(size_buffers(d, c));
+    B2C_TRY(choose_pipelined(d, c));
+    B2C_TRY(upload(d, c));
+    B2C_TRY(run_streaming_stage(d, c));
+    B2C_TRY(fill_beam_args(d, c));
+    B2C_TRY(plan_call(d, c));
+    if (c.plan.bounds.size() > 2) B2C_TRY(enqueue_chunked(d, c));
+    B2C_TRY(enqueue_plain(d, c));
+    B2C_TRY(read_back(d, c));
+    B2C_TRY(retry_failed(d, c));
+    B2C_TRY(record_timings(d, c));
+    assemble(d, c, res.get());
+    c.hp.mark(4);                                 // statistics read-back, result assembly
+    if (c.k.host_prof)
+        std::fprintf(stderr, "[b2c host ms] enqueue=%.3f wait_prepare=%.3f plan=%.3f wait_beam=%.3f assemble=%.3f\n", c.hp.ms[0],
+                     c.hp.ms[1], c.hp.ms[2], c.hp.ms[3], c.hp.ms[4]);
     *out = res.release();
     return 0;
+}
+
+int b2c_decode_batch(b2c_decoder_t* d, const void* const* logits, const int32_t* T, int n_utts, int dtype, int is_device,
+                     const b2c_decode_opts_t* opts, b2c_result_t** out) {
+    if (!d || !opts || !out || n_utts < 0 || (n_utts > 0 && (!logits || !T))) return fail(B2C_E_ARG, "null argument");
+    std::lock_guard<std::mutex> call_lock(d->call_mu);      // one call at a time per handle (any number of threads may call)
+    int rc = decode_batch_locked(d, logits, T, n_utts, dtype, is_device, opts, out, true);
+    // a pipelined attempt that could not be planned, or that met probability input (decided after the fact): plain call
+    if (rc == B2C_E_RETRY_PLAIN) rc = decode_batch_locked(d, logits, T, n_utts, dtype, is_device, opts, out, false);
+    return rc;
 }
 
 // ---- results ------------------------------------------------------------------------------
