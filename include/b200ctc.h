@@ -242,6 +242,7 @@ typedef struct {
     long long cand_hist[7];    /* frames with more than 128,256,...,4096 candidates; [6] = frames counted */
     long long inplace_frames;  /* single-token frames that updated the beam table in place (b2c_fast_cheap_step) */
     long long sorted_frames;   /* multi-token frames ranked by binary search, no grouping (b2c_fast_sorted_step) */
+    long long single_frames;   /* one-token frames after a multi-token frame, one candidate per thread (b2c_fast_single_step) */
     int hinted;                /* 1: the beam kernel was planned from the previous call's statistics and launched without
                                   waiting for this call's (no mid-call synchronisation); same results either way */
 } b2c_timings_t;

@@ -77,6 +77,7 @@ class Timings(C.Structure):
         ("cand_hist", C.c_longlong * 7),
         ("inplace_frames", C.c_longlong),
         ("sorted_frames", C.c_longlong),
+        ("single_frames", C.c_longlong),
         ("hinted", C.c_int),
     ]
 

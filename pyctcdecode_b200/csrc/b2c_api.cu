@@ -171,7 +171,8 @@ struct B2cBeamArgs {
     int gate_n;
     int gate_bounds[5];
     u64* phase_clk;            // [16] profiling builds only (-DB2C_PHASE_CLOCKS)
-    u32* m_stats;              // [8] frames over 128..4096 candidates, total frames (adaptive sizing), in-place frames, sorted (no-merge) frames
+    u32* m_stats;              // [12] frames over 128..4096 candidates, total frames (adaptive sizing), in-place frames, sorted (no-merge)
+                               // frames, utterances too wide for a one-warp CTA, utterances, single-token-step frames
 };
 
 // kFast: every frame of every utterance handed to this launch fits the shared-memory candidate
@@ -733,7 +734,7 @@ struct Geometry {
 };
 // the B200CTC_* switches (INTEGRATION.md §3), read at every call so that tests can change them between calls
 struct Knobs {
-    bool host_prof, no_pipe, no_hinted, force_v5, no_v5, no_lean, force_lean, pipe_all, no_gate, gate_early;
+    bool host_prof, no_pipe, no_hinted, force_v5, no_v5, no_lean, force_lean, pipe_all, no_gate, gate_early, no_single;
     int v5_variant, force_chunks;  // v5_variant -1: chosen from the hint
 };
 static bool env_set(const char* name) { return std::getenv(name) != nullptr; }
@@ -751,6 +752,7 @@ static Knobs read_knobs() {
     k.force_chunks = fc ? std::atoi(fc) : 0;              // tests
     k.pipe_all = env_set("B200CTC_PIPELINE_ALL"); k.no_gate = env_set("B200CTC_NO_GATE");
     k.gate_early = env_set("B200CTC_HOSTSIM_GATE_EARLY");  // hostsim tests: the later chunks of a gated launch never arrive
+    k.no_single = env_set("B200CTC_NO_SINGLE_STEP");       // tests: one-token frames after multi-token frames take the general step
     return k;
 }
 struct Plan {
@@ -1524,6 +1526,7 @@ static int make_params(b2c_decoder* d, Call& c) {
     P.alpha = d->alpha; P.beta = d->beta; P.unk_offset = d->unk;
     P.log_base_change = 0x1.26bb1bbb55516p+1;  // 1.0 / math.log10(math.e) (constants.py:18)
     P.score_boundary = d->score_boundary; P.hot_weight = o->hotword_weight; P.bucket_scale = b2c_bucket_scale(o->beam_prune_logp);
+    P.kflags = c.k.no_single ? B2C_FL_NO_SINGLE : 0;
     P.toks = d->d_toks.as<B2cTok>();
     if (d->lm) {
         auto it = d->lm->dev.find(d->device);
@@ -1941,7 +1944,7 @@ static int read_back(b2c_decoder* d, Call& c) {
     for (int q = 0; q < 6; ++q) d->hint_over[q] = ms[q];
     d->hint_frames = ms[6];
     for (int q = 0; q < 7; ++q) d->tm.cand_hist[q] = ms[q];
-    d->tm.inplace_frames = ms[7]; d->tm.sorted_frames = ms[8];
+    d->tm.inplace_frames = ms[7]; d->tm.sorted_frames = ms[8]; d->tm.single_frames = ms[11];
     d->hint_wide_utts = ms[9]; d->hint_utts = ms[10];
     d->tm.oversize_frames = 0;
     for (int q = 0; q < 6; ++q)
@@ -1994,8 +1997,8 @@ static int record_timings(b2c_decoder* d, const Call& c) {
     {
         u64 hc[32];
         CUDA_OK(cudaMemcpy(hc, d->d_clk.p, sizeof(hc), cudaMemcpyDeviceToHost));
-        std::fprintf(stderr, "[b2c phase clocks, summed over CTAs, Mcycles]");
-        for (int q = 0; q < 24; ++q) std::fprintf(stderr, " p%d=%.3f", q, hc[q] / 1e6);
+        std::fprintf(stderr, "[b2c phase clocks, summed over CTAs, cycles or frames]");
+        for (int q = 0; q < 32; ++q) std::fprintf(stderr, " p%d=%llu", q, static_cast<unsigned long long>(hc[q]));
         std::fprintf(stderr, "  frames=%llu\n", static_cast<unsigned long long>(c.g.total_frames));
     }
 #endif

@@ -61,7 +61,7 @@ struct B2cScalars {
     u32 m_inplace;       // frames handled by b2c_inplace_step
     u32 clean_s, clean_g; // leading slots of the shared-memory / HBM tier's grouping table that are known to be clear
 };
-enum { B2C_FL_BPE = 1, B2C_FL_PRUNE = 2, B2C_FL_LM = 4, B2C_FL_PSCORE = 8 };
+enum { B2C_FL_BPE = 1, B2C_FL_PRUNE = 2, B2C_FL_LM = 4, B2C_FL_PSCORE = 8, B2C_FL_NO_SINGLE = 16 };
 
 #define B2C_NBUCKET 256      // score buckets of the O(m) ranking (monotone in the score)
 #define B2C_NBUCKET_WIDE 2048 // the same for launches that rank hundreds to thousands of candidates per frame (general kernel,
@@ -1105,6 +1105,7 @@ B2C_HDN void b2c_utt_begin(B2cParams P, B2cWork W, const B2cLmState* start_state
         if (P.prune_history) fl |= B2C_FL_PRUNE;
         if (P.lm.order > 0) fl |= B2C_FL_LM;
         if (P.n_hot > 0 || P.lm.order > 0) fl |= B2C_FL_PSCORE;
+        fl |= static_cast<u32>(P.kflags) & B2C_FL_NO_SINGLE;
         sc->flags = fl;
         B2cText root;
         for (int w = 0; w < B2C_MAX_HIST; ++w) { root.win[w] = 0; root.st.words[w] = 0; root.st.backoff[w] = 0.0f; }

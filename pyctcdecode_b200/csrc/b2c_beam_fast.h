@@ -25,7 +25,7 @@
 // Frames with more than CAP candidates (or more than B2C_FAST_KS tokens) are rare on ASR-like
 // posteriors; they take the general out-of-line step on the HBM candidate tier (b2c_fast_slow_step).
 //
-// Four kinds of frame steps, chosen per frame from block-uniform facts (token count, the previous frame's
+// Five kinds of frame steps, chosen per frame from block-uniform facts (token count, the previous frame's
 // token, mode flags):
 //   b2c_fast_cheap_step   one token after a one-token frame (same token / blank / plain character without LM and
 //                         hotwords): nothing can merge, reorder or be pruned -> the table is updated in place
@@ -33,9 +33,13 @@
 //                         only if they keep slot order and threshold
 //   b2c_fast_sorted_step  K >= 2 tokens after a one-token frame, no LM / hotwords / space: the candidates are K
 //                         sorted lists that cannot merge -> ranks by search, one commit per thread
+//   b2c_fast_single_step  one token (blank / plain character) after a multi-token frame, no LM / hotwords: the
+//                         general step with one candidate per thread and its fields in registers; frames where
+//                         nothing merges or is pruned leave after one vote, without the fold and the ranking
 //   b2c_fast_step         everything else: expand + group | fold + fuse + bucket | threshold + rank + commit
-// Every special step re-checks what float64 rounding could change and falls back to b2c_fast_step on the untouched
-// state, so all three give the reference's result (tests: special_step_cases, hostsim work-item-order replay).
+// Every special step re-checks what float64 rounding could change (or what it does not handle) and falls back to
+// b2c_fast_step on the untouched state, so all of them give the reference's result (tests: special_step_cases,
+// tests/single_step.py, hostsim work-item-order replay).
 //
 // Reference lines restated: decoder.py:443-554 (frame loop), :211-224 (merge), :346-424 (LM
 // fusion), :545-554 (threshold, top-N, history prune).  Order-dependence notes: b2c_beam.h.
@@ -1141,6 +1145,335 @@ B2C_HD bool b2c_fast_sorted_step(const B2cParams& P, B2cFastSmem<WC, CAP, LT>& S
     return true;
 }
 
+// -----------------------------------------------------------------------------------------
+// one token after a multi-token frame: the general step with one candidate per thread.
+//
+// Regular alphabet, no LM, no hotwords, the token is the blank or an ordinary character (branch (i) or (iv) of
+// decoder.py:452-534 for every beam).  Candidate b comes from slot b; its thread keeps liveness, branch, new partial
+// word and own logit sum in registers across the three phases, so only the merge keys (ckey) and the own sums (cfold)
+// go to shared memory, where group mates read them.  Beams DO merge here: X.c from token c of the previous frame meets
+// X + c from its blank, and beams that differ only in their last character meet on the blank.
+//   phase 1  expand, merge key, group (only joiners pay the extent atomics); with prune_history the history keys go
+//            into the same grouping table as tagged entries.  One vote: a merge, a history-key collision or a slot
+//            below the threshold?  If none, every beam maps to one new beam in the same order (lm_score ==
+//            logit_score + 0, the same p added to every beam) and the table is updated IN PLACE (no-merge exit).
+//   phase 2  the leader (lowest index) of a group folds it left to right; its members are the claimer and the
+//            extremes ht_min / ht_max, so a group of up to three needs no scan.  The last member's fields are rebuilt
+//            from row `last` of the current table and the frame's token.  Bucket insert, per-warp maximum.
+//   phase 3  bucket prefix, in-bucket rank walk, threshold, history-prune insert and commit, from registers.
+// A group of four or more members hands the frame, state untouched, to b2c_fast_step.  Returns 0 (handed over),
+// 1 (new table in the other half: the caller flips parity) or 2 (updated in place).
+// -----------------------------------------------------------------------------------------
+// Compiled into the two-CTA variant with the resident label table only (CAP 1024, V <= LT: the no-LM workloads of
+// up to 264 utterances per H100).  In the 128- and 168-register variants the step's live state spilled and slowed the
+// LM workloads that run there and never take it (C3 beam kernel +5.7 %).
+template <int CAP, int LT>
+constexpr bool b2c_fast_has_single() { return CAP >= 1024 && LT > 0; }
+
+template <int WC, int CAP, int LT>
+B2C_HD bool b2c_fast_single_ok(const B2cFastSmem<WC, CAP, LT>& S, int sb, int slot, int K, u32 prev_single) {
+    if (!b2c_fast_has_single<CAP, LT>() || K != 1 || prev_single != B2C_NONE_U32) return false;
+    if (S.sc.flags & (B2C_FL_PSCORE | B2C_FL_BPE | B2C_FL_NO_SINGLE)) return false;
+    return (b2c_fast_tok<WC, CAP, LT>(S, sb, slot, 0).flags & B2C_TF_SPACE) == 0;
+}
+
+struct B2cSingleItem {       // what the thread of slot b keeps of its candidate across the phases of b2c_fast_single_step
+    double lg;               // own logit sum; after phase 2 (leaders): the folded logit_score
+    u64 nph;                 // new partial-word hash (after phase 2: of the group's last member)
+    u32 slots;               // grouping-table slot of the merge key | slot of the history key << 16
+    u32 meta;                // new partial length | branch (iv) << 16 | live << 17 | group leader << 18 | last member << 19
+};
+enum { B2C_SI_T3 = 1u << 16, B2C_SI_LIVE = 1u << 17, B2C_SI_LEAD = 1u << 18, B2C_SI_LAST = 19 };
+// the barrier of a phase that also ORs a per-thread flag over the block (hostsim: v was accumulated over every item)
+B2C_HD u32 b2c_sync_or(u32 v) {
+#if defined(__CUDA_ARCH__)
+    return static_cast<u32>(__syncthreads_or(static_cast<int>(v)));
+#else
+    return v;
+#endif
+}
+
+template <int WC, int CAP, int LT>
+B2C_HD int b2c_fast_single_step(const B2cParams& P, B2cFastSmem<WC, CAP, LT>& S, B2cChain* chain_arena, int par, int t, int sb,
+                                int slot) {
+    typedef B2cFastSmem<WC, CAP, LT> SM;
+    B2cFastTab<WC>& cur = S.tab[par];
+    B2cFastTab<WC>& nx = S.tab[par ^ 1];
+    const u32 n = b2c_max_slots(S.wtop);            // <= WC: at most one candidate per thread
+    const bool prune = (S.sc.flags & B2C_FL_PRUNE) != 0;
+    const bool holes = S.holes != 0;
+    const double ref = b2c_key_f64(b2c_max_slots(S.wmax));
+    constexpr u32 hmask = SM::HT - 1, ptmask = SM::PT - 1;
+    constexpr u32 PTAG = 0x80000000u;                // grouping-table entry of a history key (phase 1 only)
+    const B2cTok& ti = b2c_fast_tok<WC, CAP, LT>(S, sb, slot, 0);
+    const u32 canon = ti.canon;
+    const bool blank = (ti.flags & B2C_TF_BLANK) != 0;
+    const double p = S.rlp[slot][0];
+    // the in-place form: slot 0 (rank 0 of the previous frame, always live) stays the best, the threshold hangs on it
+    const bool t0 = blank || cur.last_tok[0] == canon;
+    const double top = b2c_combine_score(false, cur.logit[0] + p, cur.lm_hw[0], t0 ? cur.pscore[0] : 0.0, 0u);
+#if defined(__CUDA_ARCH__)
+    B2cSingleItem items[1];
+#define B2C_SITEM(b) items[0]
+#else
+    B2cSingleItem items[WC];
+#define B2C_SITEM(b) items[b]
+#endif
+
+    // ---- phase 1: expand, merge key, grouping, history key; vote for the in-place form -------------
+    B2C_FOR(s, B2C_NBUCKET) { S.bcnt[s] = 0; S.bhead[s] = B2C_NONE_U32; }
+    u32 vote = 0;
+    B2C_FOR(b, n) {
+        B2cSingleItem& it = B2C_SITEM(b);
+        const u32 ub = static_cast<u32>(b);
+        it.meta = 0;
+        if (holes && S.pt_min[S.pslot[b]] != ub) continue;
+        const u64 ph = cur.part_hash[b];
+        const u32 plen = cur.part_len[b];
+        const bool t3 = !blank && cur.last_tok[b] != canon;
+        it.nph = t3 ? b2c_hash_append(ph, ti.raw_hash, ti.raw_pow) : ph;
+        const u32 nplen = t3 ? plen + ti.raw_nchars : plen;
+        it.lg = cur.logit[b] + p;
+        S.cfold[b] = it.lg;
+        const u64 key = b2c_fast_key(cur.text_hash[b], it.nph, nplen, canon);
+        S.ckey[b] = key;
+        u64 hk = 0;
+        if (prune) {
+            hk = b2c_fast_key(cur.hist_hash[b], it.nph, nplen & 0xFFFFu, canon);
+            S.phk[b] = hk;
+        }
+        b2c_fence_block();
+        u32 hs = static_cast<u32>(key) & hmask;
+        bool claimed = false;
+        while (true) {
+            const u32 rep = b2c_atomic_cas_u32(&S.ht_idx[hs], B2C_NONE_U32, ub);
+            if (rep == B2C_NONE_U32) { claimed = true; break; }
+            b2c_fence_block();
+            if (!(rep & PTAG) && S.ckey[rep] == key) break;
+            hs = (hs + 1) & hmask;
+        }
+        if (!claimed) {
+            b2c_atomic_min_u32(&S.ht_min[hs], ub);
+            b2c_atomic_max_u32(&S.ht_max[hs], ub);
+            if (b2c_atomic_add_u32(&S.ht_cnt[hs], 1u) >= 2u) b2c_atomic_or_u32(&S.cheap_bad, 1u);    // a fourth member
+            vote = 1;
+        }
+        u32 psl = SM::HT;
+        if (prune) {       // two live beams with one history key: the later one is pruned, so not in place
+            u32 q = static_cast<u32>(hk) & hmask;
+            while (true) {
+                const u32 rep = b2c_atomic_cas_u32(&S.ht_idx[q], B2C_NONE_U32, ub | PTAG);
+                if (rep == B2C_NONE_U32) { psl = q; break; }
+                b2c_fence_block();
+                if ((rep & PTAG) && S.phk[rep & ~PTAG] == hk) { vote = 1; break; }
+                q = (q + 1) & hmask;
+            }
+        }
+        it.slots = hs | (psl << 16);
+        it.meta = (nplen & 0xFFFFu) | (t3 ? B2C_SI_T3 : 0u) | B2C_SI_LIVE;
+        const double sco = b2c_combine_score(false, it.lg, cur.lm_hw[b], t3 ? 0.0 : cur.pscore[b], nplen);
+        if (!(sco >= top + P.prune_logp)) vote = 1;
+    }
+    vote = b2c_sync_or(vote);
+
+    if (!vote) {
+        // ---- no merge, no history-key collision, every slot above the threshold: in place (b2c_fast_run_step) --
+        B2C_FOR(b, n) {
+            const B2cSingleItem& it = B2C_SITEM(b);
+            if (!(it.meta & B2C_SI_LIVE)) {     // dead slots keep their place in the score order: only their logit follows
+                cur.logit[b] = cur.logit[b] + p;
+                continue;
+            }
+            S.ht_idx[it.slots & 0xFFFFu] = B2C_NONE_U32;
+            S.ht_idx[it.slots >> 16] = B2C_NONE_U32;
+            const int ps0 = cur.pf_s[b], pe0 = cur.pf_e[b];
+            cur.logit[b] = it.lg;
+            cur.last_tok[b] = static_cast<u16>(canon);
+            if (!(it.meta & B2C_SI_T3)) {
+                if (!blank) cur.pf_e[b] = t + 1;
+            } else {
+                const u32 id = static_cast<u32>(t) * static_cast<u32>(WC) + static_cast<u32>(b);
+                B2cChain c;
+                c.parent = cur.chain[b];
+                c.tok = static_cast<u16>(S.rid[slot][0]);
+                c.kind = B2C_CK_CONT;
+                c.has_word = 0;
+                c.ws = ps0;
+                c.we = pe0;
+                b2c_chain_store(chain_arena, id, c, P.narrow_chain != 0);
+                cur.chain[b] = id;
+                cur.part_hash[b] = it.nph;
+                cur.part_len[b] = static_cast<u16>(it.meta);
+                cur.pscore[b] = 0.0;
+                cur.pf_s[b] = ps0 < 0 ? t : ps0;
+                cur.pf_e[b] = t + 1;
+            }
+        }
+        B2C_FOR(w, B2C_FAST_NW) { S.wmax[w] = w == 0 ? b2c_f64_key(top) : 0ull; }
+        B2C_FMARK(24);
+        return 2;
+    }
+    if (S.cheap_bad) {      // block-uniform, rare: a group of four or more -- the general step on the untouched state
+        B2C_FOR(b, n) {
+            const B2cSingleItem& it = B2C_SITEM(b);
+            if (!(it.meta & B2C_SI_LIVE)) continue;
+            const u32 hs = it.slots & 0xFFFFu;
+            S.ht_idx[hs] = B2C_NONE_U32;
+            S.ht_min[hs] = B2C_NONE_U32;
+            S.ht_max[hs] = 0;
+            S.ht_cnt[hs] = 0;
+            S.ht_idx[it.slots >> 16] = B2C_NONE_U32;
+        }
+        B2C_SYNC();
+        B2C_LEADER { S.cheap_bad = 0; }
+        return 0;
+    }
+
+    // ---- phase 2: fold (decoder.py:211-224), score, bucket, max -----------------------------------
+    if (holes) {   // the validity tests of phase 1 are done: release the previous frame's prune entries
+        B2C_FOR(r, n) {
+            const u32 s = S.pslot[r];
+            S.pt_idx[s] = B2C_NONE_U32;
+            S.pt_min[s] = B2C_NONE_U32;
+        }
+    }
+    {
+        u64 tmax = 0;
+        B2C_FOR(b, n) {
+            B2cSingleItem& it = B2C_SITEM(b);
+            if (!(it.meta & B2C_SI_LIVE)) continue;
+            const u32 ub = static_cast<u32>(b);
+            const u32 hs = it.slots & 0xFFFFu;
+            const u32 c0 = S.ht_idx[hs];
+            const u32 cnt = S.ht_cnt[hs] + 1;
+            u32 first = c0, last = c0, mid = c0;
+            if (cnt > 1) {      // members: the claimer c0 and the joiners ht_min <= ht_max (equal for a pair)
+                const u32 lo = S.ht_min[hs], hi = S.ht_max[hs];
+                first = lo < c0 ? lo : c0;
+                last = hi > c0 ? hi : c0;
+                mid = c0 + lo + hi - first - last;
+            }
+            if (first != ub) continue;
+            double s = it.lg;
+            if (cnt == 3) s = b2c_sum_log_scores_ool(s, S.cfold[mid]);
+            if (cnt > 1) s = b2c_sum_log_scores_ool(s, S.cfold[last]);
+            it.lg = s;
+            u32 meta = it.meta;
+            if (last != ub) {   // the merged beam takes the last member's branch and fields
+                const u64 ph = cur.part_hash[last];
+                const u32 plen = cur.part_len[last];
+                const bool t3 = !blank && cur.last_tok[last] != canon;
+                it.nph = t3 ? b2c_hash_append(ph, ti.raw_hash, ti.raw_pow) : ph;
+                meta = ((t3 ? plen + ti.raw_nchars : plen) & 0xFFFFu) | (t3 ? B2C_SI_T3 : 0u) | B2C_SI_LIVE;
+            }
+            it.meta = meta | B2C_SI_LEAD | (last << B2C_SI_LAST);
+            const u32 nplen = meta & 0xFFFFu;
+            const double sco = b2c_combine_score(false, s, cur.lm_hw[last], (meta & B2C_SI_T3) ? 0.0 : cur.pscore[last], nplen);
+            const u64 key = b2c_f64_key(sco);
+            S.ckey[b] = key;
+            const u32 bkt = b2c_bucket(ref, sco, P.bucket_scale);
+            b2c_atomic_add_u32(&S.bcnt[bkt], 1u);
+#if defined(__CUDA_ARCH__)
+            S.cnext[b] = atomicExch(&S.bhead[bkt], ub);
+#else
+            S.cnext[b] = S.bhead[bkt];
+            S.bhead[bkt] = ub;
+#endif
+            if (key > tmax) tmax = key;
+        }
+        b2c_warp_max_u64_slot(tmax, S.wmax);
+    }
+    B2C_SYNC();
+
+    // ---- phase 3: threshold (:545-546), stable top-N (:548), history prune (:550-552), commit ------
+    u32* const bpre = S.bpre[b2c_warp_id()];
+    b2c_bucket_scan_warp_v(S.bcnt, bpre);
+    const double thr = b2c_key_f64(b2c_max_slots(S.wmax)) + P.prune_logp;
+    const u32 width = static_cast<u32>(P.beam_width);
+    {
+        u32 my_top = 0;
+        B2C_FOR(b, n) {
+            const B2cSingleItem& it = B2C_SITEM(b);
+            if (!(it.meta & B2C_SI_LIVE)) continue;
+            {
+                const u32 hs = it.slots & 0xFFFFu;
+                S.ht_idx[hs] = B2C_NONE_U32;
+                S.ht_min[hs] = B2C_NONE_U32;
+                S.ht_max[hs] = 0;
+                S.ht_cnt[hs] = 0;
+                S.ht_idx[it.slots >> 16] = B2C_NONE_U32;
+            }
+            if (!(it.meta & B2C_SI_LEAD)) continue;
+            const u64 key = S.ckey[b];
+            const double sco = b2c_key_f64(key);
+            if (!(sco >= thr)) continue;
+            const u32 bkt = b2c_bucket(ref, sco, P.bucket_scale);
+            u32 rank = bpre[bkt];
+            if (rank >= width) continue;
+            for (u32 j = S.bhead[bkt]; j != B2C_NONE_U32;) {
+                const u64 kj = S.ckey[j];
+                const u32 jn = S.cnext[j];
+                const u32 gt = kj > key ? 1u : 0u, eq_before = (kj == key ? 1u : 0u) & (j < static_cast<u32>(b) ? 1u : 0u);
+                rank += gt | eq_before;
+                j = jn;
+            }
+            if (rank >= width) continue;
+            if (rank + 1 > my_top) my_top = rank + 1;
+            const u32 bl = it.meta >> B2C_SI_LAST;
+            const u32 nplen = it.meta & 0xFFFFu;
+            const bool t3 = (it.meta & B2C_SI_T3) != 0;
+            const u64 hh = cur.hist_hash[bl];
+            if (prune) {
+                const u64 hk = b2c_fast_key(hh, it.nph, nplen, canon);
+                S.phk[rank] = hk;
+                b2c_fence_block();
+                u32 q = static_cast<u32>(hk) & ptmask;
+                while (true) {
+                    const u32 rep = b2c_atomic_cas_u32(&S.pt_idx[q], B2C_NONE_U32, rank);
+                    if (rep == B2C_NONE_U32) break;
+                    b2c_fence_block();
+                    if (S.phk[rep] == hk) break;
+                    q = (q + 1) & ptmask;
+                }
+                S.pslot[rank] = q;
+                b2c_atomic_min_u32(&S.pt_min[q], rank);
+            }
+            // rank becomes beam `rank` of the next frame (decoder.py:452-534 metadata, as b2c_fast_commit)
+            const int ps0 = cur.pf_s[bl], pe0 = cur.pf_e[bl];
+            u32 chain = cur.chain[bl];
+            if (t3) {
+                const u32 id = static_cast<u32>(t) * static_cast<u32>(WC) + rank;
+                B2cChain c;
+                c.parent = chain;
+                c.tok = static_cast<u16>(S.rid[slot][0]);
+                c.kind = B2C_CK_CONT;
+                c.has_word = 0;
+                c.ws = ps0;
+                c.we = pe0;
+                b2c_chain_store(chain_arena, id, c, P.narrow_chain != 0);
+                chain = id;
+            }
+            nx.logit[rank] = it.lg;
+            nx.text_hash[rank] = cur.text_hash[bl];
+            nx.part_hash[rank] = it.nph;
+            nx.part_len[rank] = static_cast<u16>(nplen);
+            nx.last_tok[rank] = static_cast<u16>(canon);
+            nx.pf_s[rank] = !t3 ? ps0 : (ps0 < 0 ? t : ps0);
+            nx.pf_e[rank] = (!t3 && blank) ? pe0 : t + 1;
+            nx.chain[rank] = chain;
+            nx.text_node[rank] = cur.text_node[bl];
+            nx.lm_hw[rank] = cur.lm_hw[bl];
+            nx.hist_hash[rank] = hh;
+            nx.pscore[rank] = t3 ? 0.0 : cur.pscore[bl];
+        }
+        b2c_warp_max_u32_slot(my_top, S.wtop);         // the selected ranks are exactly 0 .. max(wtop)-1
+    }
+#undef B2C_SITEM
+    B2C_LAST_THREAD { S.holes = prune ? 1u : 0u; }
+    B2C_FMARK(24);
+    return 1;
+}
+
 // squeeze the dead slots out of the current table (into the other one: the caller flips its parity) and
 // leave the state the general helpers expect: sc.n_beams / sc.prev_max set, prune table clear
 template <int WC, int CAP, int LT>
@@ -1457,6 +1790,18 @@ B2C_HD void b2c_beam_block_fast(const B2cBeamArgs& A, int slot_cta, u8* smem) {
                         B2C_LAST_THREAD { ++st_sorted; }
                         B2C_FMARK(7);
                     }
+                } else if (b2c_fast_has_single<CAP, LT>() && kind == B2C_CHEAP_NO &&
+                           b2c_fast_single_ok<WC, CAP, LT>(S, sb, slot, K, prev_single)) {
+                    const int r = b2c_fast_single_step<WC, CAP, LT>(A.P, S, chain_arena, par, t, sb, slot);
+                    if (r > 0) {
+                        done_frames = 1;
+                        in_place = r == 2;
+                        // counted in global memory: one more loop-carried register costs spills in some variants
+                        if (A.m_stats) { B2C_LAST_THREAD { b2c_atomic_add_u32(A.m_stats + 11, 1u); } }
+                    }
+#if defined(B2C_PHASE_CLOCKS) && defined(__CUDA_ARCH__)
+                    if (threadIdx.x == 0) S.pclk[r == 0 ? 27 : (r == 2 ? 26 : 25)] += 1;   // handed over / no-merge exit / three phases
+#endif
                 }
                 if (done_frames == 0) {
 #if defined(B2C_PHASE_CLOCKS) && defined(__CUDA_ARCH__)
@@ -1464,10 +1809,11 @@ B2C_HD void b2c_beam_block_fast(const B2cBeamArgs& A, int slot_cta, u8* smem) {
 #endif
                     b2c_fast_step<WC, CAP, LT>(A.P, S, chain_arena, text_arena, text_cap, par, t, sb, slot, K);
 #if defined(B2C_PHASE_CLOCKS) && defined(__CUDA_ARCH__)
-                    if (threadIdx.x == 0) {      // general frames by token count: cycles in 9..11, frames in 12..14
-                        const int cls = K == 1 ? 0 : (K == 2 ? 1 : 2);
-                        S.pclk[9 + cls] += static_cast<u64>(clock64() - c0);
-                        S.pclk[12 + cls] += 1;
+                    if (threadIdx.x == 0) {      // general frames by token count: cycles in 9..11, frames in 12..14;
+                        // one token after a one-token frame (the space, LM / BPE frames): cycles in 15, frames in 23
+                        const u64 dc = static_cast<u64>(clock64() - c0);
+                        if (K == 1 && prev_single != B2C_NONE_U32) { S.pclk[15] += dc; S.pclk[23] += 1; }
+                        else { const int cls = K == 1 ? 0 : (K == 2 ? 1 : 2); S.pclk[9 + cls] += dc; S.pclk[12 + cls] += 1; }
                     }
 #endif
                     done_frames = 1;

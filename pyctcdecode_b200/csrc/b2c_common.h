@@ -190,7 +190,7 @@ struct B2cParams {
     const B2cTok* toks;
     B2cLmView lm;
     int n_lm;                  // 0: none, 1: one model, > 1: MultiLanguageModel (general kernel only)
-    int pad_lm;
+    int kflags;                // extra B2C_FL_* mode bits set by the host (B2C_FL_NO_SINGLE: B200CTC_NO_SINGLE_STEP)
     const B2cLmExtra* lmx;     // [n_lm - 1] models 1.. (device memory; the parameter block stays small: it is copied
                                // into every out-of-line call of the hot kernels)
 };
