@@ -130,6 +130,13 @@ int b2c_decoder_add_lm(b2c_decoder_t* dec, b2c_lm_t* lm);
 int b2c_decoder_set_params_lm(b2c_decoder_t* dec, int lm_index, double alpha, double beta, double unk_score_offset,
                               int lm_score_boundary);
 
+/* One hotword set (HotwordScorer, language_model.py:152-189): what opts->hotwords / hotword_weight give a whole call. */
+typedef struct {
+    const char* const* hotwords; /* raw hotword strings, split on whitespace */
+    int n_hotwords;
+    double hotword_weight;
+} b2c_hotword_set_t;
+
 typedef struct {
     int beam_width;            /* DEFAULT_BEAM_WIDTH 100          (constants.py:8)  */
     double beam_prune_logp;    /* DEFAULT_PRUNE_LOGP -10          (constants.py:10) */
@@ -147,6 +154,13 @@ typedef struct {
                                   is_end=False; B2C_FIN_KEEP: neither -- beams keep their partial words (decoder.py:571-593) */
     int text_only;             /* decode() / decode_batch() (decoder.py:859-945 return beam.text only): word frames are
                                   neither copied back nor assembled; b2c_result_n_words is 0 */
+    /* per-utterance hotwords: utterance i is decoded exactly as a call of its own with hotwords / hotword_weight of
+     * hot_sets[utt_hot_set[i]].  utt_hot_set NULL: every utterance uses hotwords / hotword_weight above and hot_sets is
+     * not read.  B2C_E_ARG: an index outside [0, n_hot_sets), or n_hotwords > 0 together with utt_hot_set.  Utterances
+     * that share an index share one table on the device. */
+    const b2c_hotword_set_t* hot_sets;
+    int n_hot_sets;
+    const int32_t* utt_hot_set; /* NULL, or [n_utts] indices into hot_sets */
 } b2c_decode_opts_t;
 void b2c_decode_opts_default(b2c_decode_opts_t* opts);
 

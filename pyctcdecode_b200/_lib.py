@@ -33,6 +33,10 @@ class StreamState(C.Structure):
 FIN_EOS, FIN_FLUSH, FIN_KEEP = 0, 1, 2
 
 
+class HotwordSet(C.Structure):
+    _fields_ = [("hotwords", C.POINTER(C.c_char_p)), ("n_hotwords", C.c_int), ("hotword_weight", C.c_double)]
+
+
 class DecodeOpts(C.Structure):
     _fields_ = [
         ("beam_width", C.c_int),
@@ -47,6 +51,9 @@ class DecodeOpts(C.Structure):
         ("stream_states", C.POINTER(StreamState)),
         ("finalize_mode", C.c_int),
         ("text_only", C.c_int),
+        ("hot_sets", C.POINTER(HotwordSet)),
+        ("n_hot_sets", C.c_int),
+        ("utt_hot_set", C.POINTER(C.c_int32)),
     ]
 
 

@@ -185,6 +185,7 @@ B2C_HD void b2c_beam_block(const B2cBeamArgs& A, int slot, u8* smem) {
     B2cWork W;
     b2c_make_work(L, smem, g, 0, kFast || L.beams_in_smem, W);
     int parity = 0;      // which beam table is current (the out-of-line step rebuilds its descriptor from it)
+    static_assert(sizeof(B2cScalars) <= 120, "the queue ticket lives behind the scalars");
     u32* s_cur = reinterpret_cast<u32*>(smem + L.s_sc + 120);  // queue ticket of this CTA
     B2C_LEADER {
         for (int q = 0; q < 6; ++q) W.sc->m_over[q] = 0;
@@ -219,7 +220,7 @@ B2C_HD void b2c_beam_block(const B2cBeamArgs& A, int slot, u8* smem) {
             sin.word_len = A.s_word_len;
             t0_frames = su.t0;
         }
-        b2c_utt_begin(A.P, W, A.start_states ? A.start_states + static_cast<u64>(u) * (A.P.n_lm > 1 ? A.P.n_lm : 1) : nullptr,
+        b2c_utt_begin(A.P, W, u, A.start_states ? A.start_states + static_cast<u64>(u) * (A.P.n_lm > 1 ? A.P.n_lm : 1) : nullptr,
                       static_cast<int>(rec.cnt), sin);
 #if defined(__CUDACC__)
 #pragma unroll 1
@@ -610,13 +611,13 @@ struct b2c_result {
     std::string pk_pieces;
 };
 
-// hotword table (language_model.py:152-189): every code-point prefix of every hotword unigram
-static void build_hot(const b2c_decode_opts_t* o, std::vector<B2cHot>& tab, int& n_hot, int& min_len_all) {
+// hotword table of one set (language_model.py:152-189): every code-point prefix of every hotword unigram; appended to
+// `tab`.  Returns the shortest hotword in code points, 0 when the set has none (then nothing is appended).
+static u32 build_hot(const char* const* words, int n_words, std::vector<B2cHot>& tab) {
     std::map<u64, std::pair<u32, u32>> pref;  // key -> (min_len, is_word)
-    n_hot = 0;
-    min_len_all = 0;
-    for (int i = 0; i < o->n_hotwords; ++i) {
-        const char* s = o->hotwords[i];
+    u32 min_len_all = 0;
+    for (int i = 0; i < n_words; ++i) {
+        const char* s = words[i];
         if (!s) continue;
         const size_t L = std::strlen(s);
         size_t p = 0;
@@ -625,9 +626,8 @@ static void build_hot(const b2c_decode_opts_t* o, std::vector<B2cHot>& tab, int&
             size_t q = p;
             while (q < L && !std::isspace(static_cast<unsigned char>(s[q]))) ++q;
             if (q > p) {
-                ++n_hot;
                 const u32 nchars = b2c_utf8_len(s + p, q - p);
-                if (min_len_all == 0 || static_cast<int>(nchars) < min_len_all) min_len_all = static_cast<int>(nchars);
+                if (min_len_all == 0 || nchars < min_len_all) min_len_all = nchars;
                 u64 h = 0;
                 for (size_t k = p; k < q; ++k) {
                     h = b2c_addmod61(b2c_mulmod61(h, B2C_HASH_BASE), static_cast<u64>(static_cast<unsigned char>(s[k])) + 1);
@@ -645,14 +645,16 @@ static void build_hot(const b2c_decode_opts_t* o, std::vector<B2cHot>& tab, int&
             p = q;
         }
     }
+    if (min_len_all == 0) return 0;
     u64 size = 16;
     while (size < pref.size() * 2 + 2) size <<= 1;
-    tab.assign(size, B2cHot{0, 0, 0});
+    B2cHot* t = &*tab.insert(tab.end(), size, B2cHot{0, 0, 0});
     for (auto& kv : pref) {
         u64 slot = b2c_mix64(kv.first) & (size - 1);
-        while (tab[slot].key != 0) slot = (slot + 1) & (size - 1);
-        tab[slot] = B2cHot{kv.first, kv.second.first, kv.second.second};
+        while (t[slot].key != 0) slot = (slot + 1) & (size - 1);
+        t[slot] = B2cHot{kv.first, kv.second.first, kv.second.second};
     }
+    return min_len_all;
 }
 
 // decode() / decode_batch() want the text only: no word vector, no frames
@@ -798,7 +800,7 @@ struct OutLayout {
 // opt-in host-side section timing (B200CTC_HOST_PROFILE=1, stderr)
 struct HostProfile {
     std::chrono::steady_clock::time_point t0 = std::chrono::steady_clock::now();
-    double ms[6] = {0, 0, 0, 0, 0, 0};
+    double ms[6] = {0, 0, 0, 0, 0, 0};     // [5]: hotword tables (make_hot), a part of [0]
     void mark(int k) { const auto now = std::chrono::steady_clock::now(); ms[k] += std::chrono::duration<double, std::milli>(now - t0).count(); t0 = now; }
 };
 
@@ -816,7 +818,10 @@ struct Call {
     bool text_only = false;       // no word lists, no frames
     std::vector<B2cStreamUtt> s_utts; std::vector<B2cStreamBeam> s_beams; std::vector<u64> s_wh; std::vector<u32> s_wl;
     B2cParams P;
-    std::vector<B2cHot> hot;
+    std::vector<B2cHotSet> hot_desc;  // [n_utts] hotword set of each utterance (make_hot)
+    std::vector<B2cHot> hot_tab;      // the tables of the call's sets, back to back
+    u64 hot_bytes = 0;
+    bool any_hot = false;             // some utterance has hotwords
     bool contiguous_dev = false;  // device input, every utterance right behind the previous one
     MetaLayout meta;
     OutLayout out;
@@ -1516,6 +1521,51 @@ static int flatten_stream_states(const b2c_decoder* d, Call& c) {
     return 0;
 }
 
+// the hotword sets of a call: one per distinct opts->utt_hot_set entry, or set 0 = opts->hotwords for every utterance.
+// d_hot holds [n_utts] B2cHotSet descriptors, then the tables of the sets that have hotwords, back to back.
+static int make_hot(b2c_decoder* d, Call& c) {
+    const auto t_start = std::chrono::steady_clock::now();
+    const b2c_decode_opts_t* o = c.opts;
+    const int n = c.g.n_utts;
+    if (o->utt_hot_set) {
+        if (o->n_hotwords > 0) return fail(B2C_E_ARG, "opts->hotwords and opts->utt_hot_set are exclusive");
+        if (o->n_hot_sets < 0 || (o->n_hot_sets > 0 && !o->hot_sets)) return fail(B2C_E_ARG, "null hot_sets");
+        for (int i = 0; i < n; ++i)
+            if (o->utt_hot_set[i] < 0 || o->utt_hot_set[i] >= o->n_hot_sets) return fail(B2C_E_ARG, "utt_hot_set index out of range");
+        for (int k = 0; k < o->n_hot_sets; ++k)
+            if (o->hot_sets[k].n_hotwords > 0 && !o->hot_sets[k].hotwords) return fail(B2C_E_ARG, "null hotwords in a hot set");
+    }
+    const int n_sets = o->utt_hot_set ? o->n_hot_sets : 1;
+    std::vector<B2cHotSet> sets(static_cast<size_t>(n_sets), B2cHotSet{nullptr, 0.0, 0u, 0u});
+    std::vector<u64> tab_off(static_cast<size_t>(n_sets), 0);
+    std::vector<char> used(static_cast<size_t>(n_sets), o->utt_hot_set ? 0 : 1);
+    for (int i = 0; o->utt_hot_set && i < n; ++i) used[o->utt_hot_set[i]] = 1;
+    c.hot_tab.clear();
+    c.any_hot = false;
+    for (int k = 0; k < n_sets; ++k) {
+        if (!used[k]) continue;
+        const char* const* words = o->utt_hot_set ? o->hot_sets[k].hotwords : o->hotwords;
+        const int n_words = o->utt_hot_set ? o->hot_sets[k].n_hotwords : o->n_hotwords;
+        sets[k].weight = o->utt_hot_set ? o->hot_sets[k].hotword_weight : o->hotword_weight;
+        tab_off[k] = c.hot_tab.size();
+        sets[k].min_len = build_hot(words, n_words, c.hot_tab);
+        if (sets[k].min_len == 0) continue;
+        sets[k].mask = static_cast<u32>(c.hot_tab.size() - tab_off[k] - 1);
+        c.any_hot = true;
+    }
+    const u64 desc_bytes = (sizeof(B2cHotSet) * static_cast<u64>(std::max(n, 1)) + 15) & ~15ull;
+    c.hot_bytes = desc_bytes + sizeof(B2cHot) * c.hot_tab.size();
+    if (d->d_hot.ensure(c.hot_bytes)) return B2C_E_NOMEM;
+    const B2cHot* dtab = reinterpret_cast<const B2cHot*>(d->d_hot.as<u8>() + desc_bytes);
+    for (int k = 0; k < n_sets; ++k)
+        if (sets[k].min_len > 0) sets[k].tab = dtab + tab_off[k];
+    c.hot_desc.resize(static_cast<size_t>(n));
+    for (int i = 0; i < n; ++i) c.hot_desc[i] = sets[o->utt_hot_set ? o->utt_hot_set[i] : 0];
+    c.P.hot_utt = d->d_hot.as<B2cHotSet>();
+    c.hp.ms[5] += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_start).count();
+    return 0;
+}
+
 // kernel parameters, the extra language models of a MultiLanguageModel, the hotword table
 static int make_params(b2c_decoder* d, Call& c) {
     const b2c_decode_opts_t* o = c.opts;
@@ -1525,7 +1575,7 @@ static int make_params(b2c_decoder* d, Call& c) {
     P.prune_logp = o->beam_prune_logp; P.token_min_logp = o->token_min_logp;
     P.alpha = d->alpha; P.beta = d->beta; P.unk_offset = d->unk;
     P.log_base_change = 0x1.26bb1bbb55516p+1;  // 1.0 / math.log10(math.e) (constants.py:18)
-    P.score_boundary = d->score_boundary; P.hot_weight = o->hotword_weight; P.bucket_scale = b2c_bucket_scale(o->beam_prune_logp);
+    P.score_boundary = d->score_boundary; P.bucket_scale = b2c_bucket_scale(o->beam_prune_logp);
     P.kflags = c.k.no_single ? B2C_FL_NO_SINGLE : 0;
     P.toks = d->d_toks.as<B2cTok>();
     if (d->lm) {
@@ -1555,10 +1605,7 @@ static int make_params(b2c_decoder* d, Call& c) {
     }
     c.g.n_lm = std::max(1, P.n_lm);
     P.hist_n = std::max(1, max_order - 1);
-    build_hot(o, c.hot, P.n_hot, P.hot_min_len_all);
-    if (d->d_hot.ensure(c.hot.size() * sizeof(B2cHot))) return B2C_E_NOMEM;
-    P.hot = d->d_hot.as<B2cHot>(); P.hot_mask = c.hot.size() - 1;
-    return 0;
+    return make_hot(d, c);
 }
 
 static bool contiguous_on_device(const Call& c) {
@@ -1611,7 +1658,7 @@ static int size_buffers(b2c_decoder* d, Call& c) {
 static int choose_pipelined(b2c_decoder* d, Call& c) {
     Geometry& g = c.g;
     g.hint_ok = d->hint_valid && d->hint_beam == g.beam_width && d->hint_lm == (c.P.lm.order > 0 ? 1 : 0) &&
-                d->hint_hot == (c.P.n_hot > 0 ? 1 : 0) && d->hint_prune == c.P.prune_history && d->hint_frames > 0;
+                d->hint_hot == (c.any_hot ? 1 : 0) && d->hint_prune == c.P.prune_history && d->hint_frames > 0;
     bool pipe = c.allow_pipe && !c.k.no_pipe && !c.is_device && !c.half_in && g.T_max >= 8 * B2C_TILE_ROWS &&
                 !g.streaming && g.n_lm == 1 && g.beam_width <= 128 && g.hint_ok && !d->pipe_refused;
     for (int i = 0; i < g.n_utts && pipe; ++i)
@@ -1672,7 +1719,10 @@ static int upload(b2c_decoder* d, Call& c) {
     CUDA_OK(cudaMemcpyAsync(c.dm, c.hm, c.meta.ord, cudaMemcpyHostToDevice, st));
     d->tm.h2d_bytes += static_cast<long long>(c.meta.bytes);
     B2C_TRY(upload_logits(d, c));
-    CUDA_OK(cudaMemcpyAsync(d->d_hot.p, c.hot.data(), c.hot.size() * sizeof(B2cHot), cudaMemcpyHostToDevice, st));
+    CUDA_OK(cudaMemcpyAsync(d->d_hot.p, c.hot_desc.data(), sizeof(B2cHotSet) * c.hot_desc.size(), cudaMemcpyHostToDevice, st));
+    if (!c.hot_tab.empty())
+        CUDA_OK(cudaMemcpyAsync(d->d_hot.as<u8>() + (c.hot_bytes - sizeof(B2cHot) * c.hot_tab.size()), c.hot_tab.data(),
+                                sizeof(B2cHot) * c.hot_tab.size(), cudaMemcpyHostToDevice, st));
     if (c.opts->lm_start_states) {
         // with a MultiLanguageModel: n_lm consecutive states per utterance (MultiLanguageModelState.states)
         std::vector<B2cLmState> start_host(static_cast<size_t>(n) * c.g.n_lm);
@@ -1940,7 +1990,7 @@ static int read_back(b2c_decoder* d, Call& c) {
     d->tm.d2h_bytes += static_cast<long long>(c.out.bytes + c.tok_bytes + (c.text_only ? 0 : c.frm_bytes) + 8ull * n + 32);
     const u32* ms = d->h_mstats.as<u32>();
     d->hint_valid = true;
-    d->hint_beam = c.opts->beam_width; d->hint_lm = c.P.lm.order > 0 ? 1 : 0; d->hint_hot = c.P.n_hot > 0 ? 1 : 0; d->hint_prune = c.P.prune_history;
+    d->hint_beam = c.opts->beam_width; d->hint_lm = c.P.lm.order > 0 ? 1 : 0; d->hint_hot = c.any_hot ? 1 : 0; d->hint_prune = c.P.prune_history;
     for (int q = 0; q < 6; ++q) d->hint_over[q] = ms[q];
     d->hint_frames = ms[6];
     for (int q = 0; q < 7; ++q) d->tm.cand_hist[q] = ms[q];
@@ -2133,8 +2183,8 @@ static int decode_batch_locked(b2c_decoder_t* d, const void* const* logits, cons
     assemble(d, c, res.get());
     c.hp.mark(4);                                 // statistics read-back, result assembly
     if (c.k.host_prof)
-        std::fprintf(stderr, "[b2c host ms] enqueue=%.3f wait_prepare=%.3f plan=%.3f wait_beam=%.3f assemble=%.3f\n", c.hp.ms[0],
-                     c.hp.ms[1], c.hp.ms[2], c.hp.ms[3], c.hp.ms[4]);
+        std::fprintf(stderr, "[b2c host ms] enqueue=%.3f wait_prepare=%.3f plan=%.3f wait_beam=%.3f assemble=%.3f hotwords=%.3f\n",
+                     c.hp.ms[0], c.hp.ms[1], c.hp.ms[2], c.hp.ms[3], c.hp.ms[4], c.hp.ms[5]);
     *out = res.release();
     return 0;
 }

@@ -52,6 +52,7 @@ struct B2cBeamTab {
 struct B2cScalars {
     u64 max_key;
     double prev_max;     // best lm_score of the previous frame: reference point of the score buckets
+    B2cHotSet hot;       // this utterance's hotword set (b2c_utt_begin; parked with the rest by chunked launches)
     u32 n_beams, n_sel, n_new, chain_used, text_used, status, force_break;
     u32 flags;           // B2C_FL_*: mode bits re-read from shared memory every frame so that the compiler
                          // cannot unswitch (= replicate) the frame loop on them
@@ -251,10 +252,10 @@ B2C_HD B2cLmState* b2c_text_states_x(const B2cText* arena, u32 text_cap, int n_l
     return reinterpret_cast<B2cLmState*>(const_cast<B2cText*>(arena) + text_cap) + static_cast<u64>(node) * static_cast<u64>(n_lm - 1);
 }
 // out_x: where the end states of models 1.. go (MultiLanguageModel; nullptr: not wanted)
-B2C_HDN void b2c_text_extend(B2cParams P, const B2cText* arena, u32 text_cap, u32 parent_id, u64 word_hash, u32 word_len, int is_eos,
-                             B2cTextNew* out, B2cLmState* out_x) {
+B2C_HDN void b2c_text_extend(B2cParams P, const B2cHotSet& H, const B2cText* arena, u32 text_cap, u32 parent_id, u64 word_hash,
+                             u32 word_len, int is_eos, B2cTextNew* out, B2cLmState* out_x) {
     const B2cText* parent = arena + parent_id;
-    out->hw_count = parent->hw_count + b2c_hot_is_word(P, word_hash, word_len);
+    out->hw_count = parent->hw_count + b2c_hot_is_word(H, word_hash, word_len);
     if (P.n_lm > 1) {
         // MultiLanguageModel.score (language_model.py:485-502): sum of the models' scores, left to right, / N
         const B2cLmState* px = b2c_text_states_x(arena, text_cap, P.n_lm, parent_id);
@@ -270,34 +271,26 @@ B2C_HDN void b2c_text_extend(B2cParams P, const B2cText* arena, u32 text_cap, u3
         }
         sc = sc / static_cast<double>(P.n_lm);
         out->raw_lm = parent->raw_lm + sc;
-        out->lm_hw = out->raw_lm + P.hot_weight * static_cast<double>(out->hw_count);
+        out->lm_hw = out->raw_lm + H.weight * static_cast<double>(out->hw_count);
     } else if (P.lm.order > 0) {
         B2cLmState in = parent->st;
         double sc = b2c_lm_score_word(P, in, word_hash, word_len, is_eos != 0, out->st);
         out->raw_lm = parent->raw_lm + sc;
-        out->lm_hw = out->raw_lm + P.hot_weight * static_cast<double>(out->hw_count);
+        out->lm_hw = out->raw_lm + H.weight * static_cast<double>(out->hw_count);
     } else {
         out->raw_lm = 0.0;
         out->st.length = 0;
-        out->lm_hw = P.hot_weight * static_cast<double>(out->hw_count);
+        out->lm_hw = H.weight * static_cast<double>(out->hw_count);
     }
 }
 
 // score of an unfinished word, scalar arguments only (no parameter block copy on this path)
-B2C_HDN double b2c_partial_score_ool(int n_hot, const B2cHot* hot, u64 hot_mask, double hot_weight, int hot_min_len_all,
-                                     int lm_order, int have_unigrams, const u64* prefixes, u64 prefix_mask,
+B2C_HDN double b2c_partial_score_ool(const B2cHotSet& H, int lm_order, int have_unigrams, const u64* prefixes, u64 prefix_mask,
                                      double unk_offset, u64 part_hash, u32 part_len) {
-    if (n_hot > 0) {
-        if (part_len == 0) return hot_weight * 0 / hot_min_len_all;
-        const u64 key = part_hash + 1;
-        u64 slot = b2c_mix64(key) & hot_mask;
-        while (true) {
-            const B2cHot* e = hot + slot;
-            const u64 k = e->key;
-            if (k == key) return hot_weight * static_cast<double>(part_len) / static_cast<double>(e->min_len);
-            if (k == 0) break;
-            slot = (slot + 1) & hot_mask;
-        }
+    if (H.min_len > 0) {
+        if (part_len == 0) return H.weight * 0 / H.min_len;
+        const B2cHot* e = b2c_hot_find(H, part_hash);
+        if (e) return H.weight * static_cast<double>(part_len) / static_cast<double>(e->min_len);
     }
     if (lm_order == 0) return 0.0;
     double is_oov = 1.0;
@@ -317,11 +310,11 @@ B2C_HDN double b2c_partial_score_ool(int n_hot, const B2cHot* hot, u64 hot_mask,
 }
 // MultiLanguageModel.score_partial_token (language_model.py:478-483): mean over the models; the hotword prefix
 // score takes precedence exactly as with one model (decoder.py:397-409)
-B2C_HDN double b2c_partial_score_multi(B2cParams P, u64 part_hash, u32 part_len) {
-    if (P.n_hot > 0) {
-        if (part_len == 0) return P.hot_weight * 0 / P.hot_min_len_all;
-        const B2cHot* h = b2c_hot_find(P, part_hash);
-        if (h) return P.hot_weight * static_cast<double>(part_len) / static_cast<double>(h->min_len);
+B2C_HDN double b2c_partial_score_multi(B2cParams P, const B2cHotSet& H, u64 part_hash, u32 part_len) {
+    if (H.min_len > 0) {
+        if (part_len == 0) return H.weight * 0 / H.min_len;
+        const B2cHot* h = b2c_hot_find(H, part_hash);
+        if (h) return H.weight * static_cast<double>(part_len) / static_cast<double>(h->min_len);
     }
     double s = b2c_lm_partial_v(P.lm, P.unk_offset, part_hash, part_len);
     for (int j = 1; j < P.n_lm; ++j) {
@@ -330,11 +323,10 @@ B2C_HDN double b2c_partial_score_multi(B2cParams P, u64 part_hash, u32 part_len)
     }
     return s / static_cast<double>(P.n_lm);
 }
-B2C_HD double b2c_partial_score_of(const B2cParams& P, bool need, u64 part_hash, u32 part_len) {
+B2C_HD double b2c_partial_score_of(const B2cParams& P, const B2cHotSet& H, bool need, u64 part_hash, u32 part_len) {
     if (!need) return 0.0;
-    if (P.n_lm > 1) return b2c_partial_score_multi(P, part_hash, part_len);
-    return b2c_partial_score_ool(P.n_hot, P.hot, P.hot_mask, P.hot_weight, P.hot_min_len_all, P.lm.order,
-                                 P.lm.have_unigrams, P.lm.prefixes, P.lm.prefix_mask, P.unk_offset, part_hash, part_len);
+    if (P.n_lm > 1) return b2c_partial_score_multi(P, H, part_hash, part_len);
+    return b2c_partial_score_ool(H, P.lm.order, P.lm.have_unigrams, P.lm.prefixes, P.lm.prefix_mask, P.unk_offset, part_hash, part_len);
 }
 
 // history-prune hash of "text + word" (last hist_n words)
@@ -347,13 +339,13 @@ B2C_HDN u64 b2c_hist_extend(const B2cText* par, int hist_n, u64 word_hash) {
 
 // a surviving beam finished a word: create the text node (LM state, raw score, hotword count, history)
 struct B2cTextCommit { u32 node; double lm_hw; u64 hist_hash; };
-B2C_HDN void b2c_commit_text(B2cParams P, B2cText* arena, u32 text_cap, u32* text_used, u32* status, u32 parent_id,
+B2C_HDN void b2c_commit_text(B2cParams P, const B2cHotSet& H, B2cText* arena, u32 text_cap, u32* text_used, u32* status, u32 parent_id,
                              u64 word_hash, u32 word_len, B2cTextCommit* out) {
     const B2cText* par = arena + parent_id;
     // the node is allocated first so that a MultiLanguageModel's other end states are written in place
     const u32 id = b2c_atomic_add_u32(text_used, 1u);
     B2cTextNew tn;
-    b2c_text_extend(P, arena, text_cap, parent_id, word_hash, word_len, 0, &tn,
+    b2c_text_extend(P, H, arena, text_cap, parent_id, word_hash, word_len, 0, &tn,
                     (P.n_lm > 1 && id < text_cap) ? b2c_text_states_x(arena, text_cap, P.n_lm, id) : nullptr);
     out->lm_hw = tn.lm_hw;
     out->node = parent_id;
@@ -693,7 +685,7 @@ B2C_HD void b2c_commit_one(const B2cParams& P, const B2cWork& W, const Tier& C, 
     u64 hh = cur.hist_hash[bl];
     if (word_len > 0) {
         B2cTextCommit tc;
-        b2c_commit_text(P, W.text, W.text_cap, &sc->text_used, &sc->status, tnode, cur.part_hash[bl], word_len, &tc);
+        b2c_commit_text(P, sc->hot, W.text, W.text_cap, &sc->text_used, &sc->status, tnode, cur.part_hash[bl], word_len, &tc);
         tnode = tc.node;
         lm_hw = tc.lm_hw;
         hh = tc.hist_hash;
@@ -703,7 +695,7 @@ B2C_HD void b2c_commit_one(const B2cParams& P, const B2cWork& W, const Tier& C, 
     nx.hist_hash[j] = hh;
     double ps = 0.0;
     if (type == 0) ps = cur.pscore[bl];
-    else if (part_len > 0) ps = b2c_partial_score_of(P, (flags & B2C_FL_PSCORE) != 0, part_hash, part_len);
+    else if (part_len > 0) ps = b2c_partial_score_of(P, sc->hot, (flags & B2C_FL_PSCORE) != 0, part_hash, part_len);
     nx.pscore[j] = ps;
 }
 
@@ -829,12 +821,12 @@ B2C_HD void b2c_frame_step(const B2cParams& P, B2cWork& W, int t, const u32* tk_
             double lm_hw = cur.lm_hw[bl];
             if ((type == 1 || type == 2) && cur.part_len[bl] > 0) {
                 B2cTextNew tn;
-                b2c_text_extend(P, W.text, W.text_cap, cur.text_node[bl], cur.part_hash[bl], cur.part_len[bl], 0, &tn, nullptr);
+                b2c_text_extend(P, sc->hot, W.text, W.text_cap, cur.text_node[bl], cur.part_hash[bl], cur.part_len[bl], 0, &tn, nullptr);
                 lm_hw = tn.lm_hw;
             }
             double ps = 0.0;
             if (type == 0) ps = cur.pscore[bl];
-            else if (part_len > 0) ps = b2c_partial_score_of(P, (flags & B2C_FL_PSCORE) != 0, cph & B2C_PH_MASK, part_len);
+            else if (part_len > 0) ps = b2c_partial_score_of(P, sc->hot, (flags & B2C_FL_PSCORE) != 0, cph & B2C_PH_MASK, part_len);
             const double sco = b2c_combine_score((flags & B2C_FL_LM) != 0, s, lm_hw, ps, part_len);
             const u64 key = b2c_f64_key(sco);
             C.ckey[i] = key;
@@ -972,7 +964,7 @@ B2C_HD bool b2c_inplace_step(const B2cParams& P, const B2cWork& W, int t, int ki
         B2C_FOR(b, n) {
             const u64 nph = b2c_hash_append(cur.part_hash[b], ti.raw_hash, ti.raw_pow);
             const u32 nplen = (static_cast<u32>(cur.part_len[b]) + ti.raw_nchars) & 0xFFFFu;
-            const double ps = b2c_partial_score_of(P, true, nph, nplen);
+            const double ps = b2c_partial_score_of(P, sc->hot, true, nph, nplen);
             union { double d; u64 u; } c;
             c.d = ps;
             Cs.ckey[b] = c.u;
@@ -1080,7 +1072,7 @@ struct B2cStreamIn {           // streaming input of one utterance (n_beams == 0
     const u64* word_hash;
     const u32* word_len;
 };
-B2C_HDN void b2c_utt_begin(B2cParams P, B2cWork W, const B2cLmState* start_state, int K_first, B2cStreamIn in) {
+B2C_HDN void b2c_utt_begin(B2cParams P, B2cWork W, int u, const B2cLmState* start_state, int K_first, B2cStreamIn in) {
     const u32 M0 = static_cast<u32>(K_first > 0 ? K_first : 1) * (in.n_beams > 0 ? in.n_beams : 1u);
     {
         const B2cCandTier C0 = b2c_pick_tier(W, M0);
@@ -1100,11 +1092,12 @@ B2C_HDN void b2c_utt_begin(B2cParams P, B2cWork W, const B2cLmState* start_state
         sc->force_break = 0;
         sc->inplace_bad = 0;
         sc->prev_max = 0.0;
+        sc->hot = P.hot_utt[u];
         u32 fl = 0;
         if (P.is_bpe) fl |= B2C_FL_BPE;
         if (P.prune_history) fl |= B2C_FL_PRUNE;
         if (P.lm.order > 0) fl |= B2C_FL_LM;
-        if (P.n_hot > 0 || P.lm.order > 0) fl |= B2C_FL_PSCORE;
+        if (sc->hot.min_len > 0 || P.lm.order > 0) fl |= B2C_FL_PSCORE;
         fl |= static_cast<u32>(P.kflags) & B2C_FL_NO_SINGLE;
         sc->flags = fl;
         B2cText root;
@@ -1142,7 +1135,7 @@ B2C_HDN void b2c_utt_begin(B2cParams P, B2cWork W, const B2cLmState* start_state
         }
         const B2cBeamTab& c = W.cur;
         c.logit[0] = 0.0;
-        c.lm_hw[0] = P.lm.order > 0 ? 0.0 : P.hot_weight * 0;
+        c.lm_hw[0] = P.lm.order > 0 ? 0.0 : sc->hot.weight * 0;
         c.pscore[0] = 0.0;
         c.text_hash[0] = B2C_TEXT_SEED;
         c.part_hash[0] = 0;
@@ -1167,11 +1160,11 @@ B2C_HDN void b2c_utt_begin(B2cParams P, B2cWork W, const B2cLmState* start_state
         const B2cStreamBeam sb = in.beams[b];
         u64 th = B2C_TEXT_SEED, hh = B2C_HIST_SEED;
         u32 node = 0;
-        double lm_hw = P.lm.order > 0 ? 0.0 : P.hot_weight * 0;
+        double lm_hw = P.lm.order > 0 ? 0.0 : sc->hot.weight * 0;
         for (u32 w = 0; w < sb.n_words; ++w) {
             const u64 wh = in.word_hash[sb.word_off + w];
             B2cTextCommit tc;
-            b2c_commit_text(P, W.text, W.text_cap, &sc->text_used, &sc->status, node, wh, in.word_len[sb.word_off + w], &tc);
+            b2c_commit_text(P, sc->hot, W.text, W.text_cap, &sc->text_used, &sc->status, node, wh, in.word_len[sb.word_off + w], &tc);
             node = tc.node;
             lm_hw = tc.lm_hw;
             hh = tc.hist_hash;
@@ -1180,7 +1173,7 @@ B2C_HDN void b2c_utt_begin(B2cParams P, B2cWork W, const B2cLmState* start_state
         const B2cBeamTab& c = W.cur;
         c.logit[b] = sb.logit;
         c.lm_hw[b] = lm_hw;
-        c.pscore[b] = sb.part_len > 0 ? b2c_partial_score_of(P, P.n_hot > 0 || P.lm.order > 0, sb.part_hash, sb.part_len) : 0.0;
+        c.pscore[b] = sb.part_len > 0 ? b2c_partial_score_of(P, sc->hot, (sc->flags & B2C_FL_PSCORE) != 0, sb.part_hash, sb.part_len) : 0.0;
         c.text_hash[b] = th;
         c.part_hash[b] = sb.part_hash;
         c.hist_hash[b] = hh;
@@ -1258,7 +1251,7 @@ B2C_HDN void b2c_finalize(B2cParams P, B2cWork W, B2cOut O, int fin_mode) {
         } else if ((P.lm.order > 0 && (is_eos || cur.part_len[last] > 0)) || cur.part_len[last] > 0) {
             // is_eos=False with an empty next_word is a cache hit on (text, False) as well
             B2cTextNew tn;
-            b2c_text_extend(P, W.text, W.text_cap, cur.text_node[last], cur.part_hash[last], cur.part_len[last], is_eos, &tn, nullptr);
+            b2c_text_extend(P, sc->hot, W.text, W.text_cap, cur.text_node[last], cur.part_hash[last], cur.part_len[last], is_eos, &tn, nullptr);
             lm_hw = tn.lm_hw;
         } else {
             lm_hw = cur.lm_hw[last];
@@ -1311,7 +1304,7 @@ B2C_HDN void b2c_finalize(B2cParams P, B2cWork W, B2cOut O, int fin_mode) {
                 }
             } else {
                 B2cTextNew tn;
-                b2c_text_extend(P, W.text, W.text_cap, cur.text_node[last], cur.part_hash[last], cur.part_len[last], is_eos, &tn,
+                b2c_text_extend(P, sc->hot, W.text, W.text_cap, cur.text_node[last], cur.part_hash[last], cur.part_len[last], is_eos, &tn,
                                 (P.n_lm > 1 && O.states_x) ? O.states_x + static_cast<u64>(r) * (P.n_lm - 1) : nullptr);
                 st = tn.st;
             }

@@ -328,12 +328,12 @@ B2C_HD void b2c_fast_commit(const B2cParams& P, B2cFastSmem<WC, CAP, LT>& S, con
     if (word_len > 0) {
         if (flags & B2C_FL_PSCORE) {
             B2cTextCommit tc;
-            b2c_commit_text(P, text_arena, text_cap, &S.sc.text_used, &S.sc.status, tnode, cur.part_hash[bl], word_len, &tc);
+            b2c_commit_text(P, S.sc.hot, text_arena, text_cap, &S.sc.text_used, &S.sc.status, tnode, cur.part_hash[bl], word_len, &tc);
             tnode = tc.node;
             lm_hw = tc.lm_hw;
             hh = tc.hist_hash;
         } else {
-            // no LM, no hotwords: hist_n == 1, the text-level score stays hot_weight * 0 and nothing ever reads
+            // no LM, no hotwords: hist_n == 1, the text-level score stays the set's weight * 0 and nothing ever reads
             // a text node other than the root -> no arena traffic on word boundaries
             hh = b2c_hist_fold(B2C_HIST_SEED, cur.part_hash[bl]);
         }
@@ -343,7 +343,7 @@ B2C_HD void b2c_fast_commit(const B2cParams& P, B2cFastSmem<WC, CAP, LT>& S, con
     nx.hist_hash[j] = hh;
     double ps = 0.0;
     if (type == 0) ps = cur.pscore[bl];
-    else if (part_len > 0) ps = b2c_partial_score_of(P, (flags & B2C_FL_PSCORE) != 0, part_hash, part_len);
+    else if (part_len > 0) ps = b2c_partial_score_of(P, S.sc.hot, (flags & B2C_FL_PSCORE) != 0, part_hash, part_len);
     nx.pscore[j] = ps;
 }
 
@@ -622,15 +622,15 @@ B2C_HD void b2c_fast_step(const B2cParams& P, B2cFastSmem<WC, CAP, LT>& S, B2cCh
             const u32 part_len = S.cmeta[last] & 0xFFFFu;
             const u32 bl = S.cbk[last] & 0xFFFFu;
             double lm_hw = cur.lm_hw[bl];
-            // without LM and hotwords the text-level score is the constant hot_weight * 0: no text node is read
+            // without LM and hotwords the text-level score is the constant weight * 0 of the empty hotword set: no text node is read
             if ((flags & B2C_FL_PSCORE) && (type == 1 || type == 2) && cur.part_len[bl] > 0) {
                 B2cTextNew tn;
-                b2c_text_extend(P, text_arena, text_cap, cur.text_node[bl], cur.part_hash[bl], cur.part_len[bl], 0, &tn, nullptr);
+                b2c_text_extend(P, S.sc.hot, text_arena, text_cap, cur.text_node[bl], cur.part_hash[bl], cur.part_len[bl], 0, &tn, nullptr);
                 lm_hw = tn.lm_hw;
             }
             double ps = 0.0;
             if (type == 0) ps = cur.pscore[bl];
-            else if (part_len > 0) ps = b2c_partial_score_of(P, (flags & B2C_FL_PSCORE) != 0, cph & B2C_PH_MASK, part_len);
+            else if (part_len > 0) ps = b2c_partial_score_of(P, S.sc.hot, (flags & B2C_FL_PSCORE) != 0, cph & B2C_PH_MASK, part_len);
             const double sco = b2c_combine_score((flags & B2C_FL_LM) != 0, s, lm_hw, ps, part_len);
             const u64 key = b2c_f64_key(sco);
             S.ckey[i] = key;
@@ -904,7 +904,7 @@ B2C_HD bool b2c_fast_scored_step(const B2cParams& P, B2cFastSmem<WC, CAP, LT>& S
     B2C_FOR(b, n) {
         const u64 nph = b2c_hash_append(cur.part_hash[b], ti.raw_hash, ti.raw_pow);
         const u32 nplen = static_cast<u32>(cur.part_len[b]) + ti.raw_nchars;
-        const double ps = b2c_partial_score_of(P, true, nph, nplen & 0xFFFFu);
+        const double ps = b2c_partial_score_of(P, S.sc.hot, true, nph, nplen & 0xFFFFu);
         union { double d; u64 u; } c;
         c.d = ps;
         S.ckey[b] = c.u;
@@ -1640,7 +1640,7 @@ B2C_HD void b2c_beam_block_fast(const B2cBeamArgs& A, int slot_cta, u8* smem) {
         } else {
             B2cWork W;
             b2c_fast_work(S, L, g, 0, false, W);
-            b2c_utt_begin(A.P, W, A.start_states ? A.start_states + u : nullptr, 1, B2cStreamIn{nullptr, 0u, nullptr, nullptr});
+            b2c_utt_begin(A.P, W, u, A.start_states ? A.start_states + u : nullptr, 1, B2cStreamIn{nullptr, 0u, nullptr, nullptr});
         }
         B2C_FOR(s, SM::HT + 1) {
             S.ht_idx[s] = B2C_NONE_U32;

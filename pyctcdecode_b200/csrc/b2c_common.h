@@ -154,6 +154,13 @@ struct B2cLmState {            // kenlm::ngram::State
 };
 
 struct B2cHot { u64 key; u32 min_len; u32 is_word; };                // hotword prefix table
+// The hotword set of one utterance (HotwordScorer, language_model.py:152-189): its prefix table, weight and shortest
+// hotword.  Utterances with equal sets share one table.  min_len == 0: no hotwords (every hotword has a code point).
+struct B2cHotSet {
+    const B2cHot* tab; double weight;
+    u32 mask;                  // table slots - 1
+    u32 min_len;               // shortest hotword (answer for the empty prefix)
+};
 
 // MultiLanguageModel (reference language_model.py:455-502): the mean of up to B2C_MAX_LMS n-gram models, each
 // with its own tables, vocabulary, unigram set and alpha / beta / unk offset / boundary flag.  Model 0 lives
@@ -182,11 +189,8 @@ struct B2cParams {
     double token_min_logp;
     double alpha, beta, unk_offset, log_base_change;
     int score_boundary;
-    int n_hot;                 // number of hotword unigrams (0: none)
-    int hot_min_len_all;       // shortest hotword (answer for the empty prefix)
-    double hot_weight;
     double bucket_scale;       // score buckets per nat for the O(m) ranking (host computed)
-    const B2cHot* hot; u64 hot_mask;
+    const B2cHotSet* hot_utt;  // [n_utts] hotword set of each utterance, copied into B2cScalars::hot by b2c_utt_begin
     const B2cTok* toks;
     B2cLmView lm;
     int n_lm;                  // 0: none, 1: one model, > 1: MultiLanguageModel (general kernel only)

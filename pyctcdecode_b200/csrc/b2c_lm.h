@@ -49,15 +49,15 @@ B2C_HD const B2cNgram* b2c_ngram_find(const B2cLmView& lm, u64 key) {
         slot = (slot + 1) & lm.ngram_mask;
     }
 }
-B2C_HD const B2cHot* b2c_hot_find(const B2cParams& P, u64 prefix_hash) {
+B2C_HD const B2cHot* b2c_hot_find(const B2cHotSet& H, u64 prefix_hash) {
     u64 key = prefix_hash + 1;
-    u64 slot = b2c_mix64(key) & P.hot_mask;
+    u64 slot = b2c_mix64(key) & H.mask;
     while (true) {
-        const B2cHot* e = P.hot + slot;
+        const B2cHot* e = H.tab + slot;
         u64 k = e->key;
         if (k == key) return e;
         if (k == 0) return nullptr;
-        slot = (slot + 1) & P.hot_mask;
+        slot = (slot + 1) & H.mask;
     }
 }
 
@@ -128,12 +128,12 @@ B2C_HD double b2c_lm_partial_v(const B2cLmView& lm, double unk_offset, u64 part_
 
 // score of an unfinished word.  LM mode (reference decoder.py:397-409): hotword prefix score
 // if the partial is a prefix of a hotword, else the LM's OOV-prefix penalty.  No-LM mode
-// (decoder.py:363-367): hotword prefix score or 0.
-B2C_HD double b2c_partial_score(const B2cParams& P, u64 part_hash, u32 part_len) {
-    if (P.n_hot > 0) {
-        if (part_len == 0) return P.hot_weight * 0 / P.hot_min_len_all;
-        const B2cHot* h = b2c_hot_find(P, part_hash);
-        if (h) return P.hot_weight * static_cast<double>(part_len) / static_cast<double>(h->min_len);
+// (decoder.py:363-367): hotword prefix score or 0.  H: the utterance's hotword set.
+B2C_HD double b2c_partial_score(const B2cParams& P, const B2cHotSet& H, u64 part_hash, u32 part_len) {
+    if (H.min_len > 0) {
+        if (part_len == 0) return H.weight * 0 / H.min_len;
+        const B2cHot* h = b2c_hot_find(H, part_hash);
+        if (h) return H.weight * static_cast<double>(part_len) / static_cast<double>(h->min_len);
     }
     if (P.lm.order == 0) return 0.0;
     double is_oov = 1.0;
@@ -143,8 +143,8 @@ B2C_HD double b2c_partial_score(const B2cParams& P, u64 part_hash, u32 part_len)
     return unk;
 }
 
-B2C_HD u32 b2c_hot_is_word(const B2cParams& P, u64 word_hash, u32 word_len) {
-    if (P.n_hot == 0 || word_len == 0) return 0;
-    const B2cHot* h = b2c_hot_find(P, word_hash);
+B2C_HD u32 b2c_hot_is_word(const B2cHotSet& H, u64 word_hash, u32 word_len) {
+    if (H.min_len == 0 || word_len == 0) return 0;
+    const B2cHot* h = b2c_hot_find(H, word_hash);
     return (h && h->is_word) ? 1u : 0u;
 }

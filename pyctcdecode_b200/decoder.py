@@ -12,6 +12,7 @@ import ctypes as C
 import dataclasses
 import logging
 import os
+import struct
 import threading
 from typing import Any, Collection, Dict, Iterable, List, NamedTuple, Optional, Sequence, Tuple, Union
 
@@ -114,6 +115,30 @@ def _cuda_index(t: Any) -> Optional[int]:
     if getattr(t, "is_cuda", False):
         return int(t.device.index if t.device.index is not None else 0)
     return None
+
+
+def _utt_hot_sets(n: int, hotwords: Optional[Iterable[str]], hotwords_list: Optional[Sequence[Optional[Iterable[str]]]],
+                  hotword_weight_list: Optional[Sequence[float]]) -> Optional[List[Tuple[List[str], float]]]:
+    """(hotwords, weight) of each of the n utterances of a call with per-utterance hotwords, None without them.
+    `hotwords` is the call-wide list, which must then be empty."""
+    if hotwords_list is None:
+        if hotword_weight_list is not None:
+            raise ValueError("hotword_weight_list needs hotwords_list")
+        return None
+    if hotwords is not None and len(list(hotwords)) > 0:
+        raise ValueError("pass either hotwords or hotwords_list, not both")
+    hotwords_list = list(hotwords_list)
+    if len(hotwords_list) != n:
+        raise ValueError("hotwords_list has %d entries for %d utterances" % (len(hotwords_list), n))
+    weights = [DEFAULT_HOTWORD_WEIGHT] * n if hotword_weight_list is None else [float(w) for w in hotword_weight_list]
+    if len(weights) != n:
+        raise ValueError("hotword_weight_list has %d entries for %d utterances" % (len(weights), n))
+    out = []
+    for words, w in zip(hotwords_list, weights):
+        if isinstance(words, (str, bytes)):
+            raise ValueError("each hotwords_list entry is None or a list of hotwords, not a string: %r" % (words,))
+        out.append(([x.strip() for x in (words or []) if len(x.strip()) > 0], w))
+    return out
 
 
 def _as_matrix(logits: Any) -> Tuple[Any, int, int, int, bool]:
@@ -283,13 +308,16 @@ class BeamSearchDecoderCTC:
              prune_history: bool, hotwords: Optional[Iterable[str]], hotword_weight: float, max_out_beams: int,
              lm_start_states: Optional[Sequence[Optional[AbstractLMState]]] = None, with_state: bool = True,
              device: Optional[int] = None, texts_only: bool = False, lengths: Optional[Sequence[int]] = None,
-             stream: Optional[Sequence[Tuple[Sequence[Beam], int]]] = None, finalize_mode: int = _lib.FIN_EOS) -> Any:
+             stream: Optional[Sequence[Tuple[Sequence[Beam], int]]] = None, finalize_mode: int = _lib.FIN_EOS,
+             hotwords_list: Optional[Sequence[Optional[Iterable[str]]]] = None,
+             hotword_weight_list: Optional[Sequence[float]] = None) -> Any:
         packed = self._as_packed_batch(logits_list)
         if lengths is not None and packed is None:
             raise ValueError("lengths= needs one padded [B, T, V] array or tensor")
         if packed is not None:
             # one [B, T, V] array / tensor: no per-utterance conversion, pointers by arithmetic
             owner, base, n, t_each, dtype_code, is_device = packed
+            utt_hot = _utt_hot_sets(n, hotwords, hotwords_list, hotword_weight_list)
             if n == 0:
                 return []
             step = t_each * len(self._idx2vocab) * {0: 4, 1: 8, 2: 2, 3: 2}[dtype_code]
@@ -304,6 +332,7 @@ class BeamSearchDecoderCTC:
             for logits in logits_list:
                 self._check_logits_dimension(logits)
             n = len(logits_list)
+            utt_hot = _utt_hot_sets(n, hotwords, hotwords_list, hotword_weight_list)
             if n == 0:
                 return []
             mats = [_as_matrix(x) for x in logits_list]
@@ -331,13 +360,14 @@ class BeamSearchDecoderCTC:
         with self._run_lock:
             return self._run_locked(mats, n, dtype_code, is_device, device, torch_stream, beam_width, beam_prune_logp,
                                     token_min_logp, prune_history, hotwords, hotword_weight, max_out_beams, lm_start_states,
-                                    with_state, texts_only, stream, finalize_mode)
+                                    with_state, texts_only, stream, finalize_mode, utt_hot)
 
     def _run_locked(self, mats: List[Tuple[Any, int, int, int, bool]], n: int, dtype_code: int, is_device: bool,
                     device: Optional[int], torch_stream: Optional[int], beam_width: int, beam_prune_logp: float,
                     token_min_logp: float, prune_history: bool, hotwords: Optional[Iterable[str]], hotword_weight: float,
                     max_out_beams: int, lm_start_states: Optional[Sequence[Optional[AbstractLMState]]], with_state: bool,
-                    texts_only: bool, stream: Optional[Sequence[Tuple[Sequence[Beam], int]]], finalize_mode: int) -> Any:
+                    texts_only: bool, stream: Optional[Sequence[Tuple[Sequence[Beam], int]]], finalize_mode: int,
+                    utt_hot: Optional[List[Tuple[List[str], float]]] = None) -> Any:
         handle = self._handle(device)
         lm = self._language_model
         L = _lib.lib()
@@ -359,6 +389,23 @@ class BeamSearchDecoderCTC:
         opts.hotwords = C.cast(hot_arr, C.POINTER(C.c_char_p))
         opts.n_hotwords = len(hot)
         opts.hotword_weight = float(hotword_weight)
+        keep_alive: List[Any] = []
+        if utt_hot is not None:
+            # utterances with the same (hotwords, weight) share one set; the weight is compared bit for bit
+            set_of: Dict[Tuple[Tuple[str, ...], bytes], int] = {}
+            index = [set_of.setdefault((tuple(words), struct.pack("<d", w)), len(set_of)) for words, w in utt_hot]
+            sets = (_lib.HotwordSet * len(set_of))()
+            for (words, wbits), k in set_of.items():
+                arr = _lib.cstr_array(list(words))
+                keep_alive.append(arr)
+                sets[k].hotwords = C.cast(arr, C.POINTER(C.c_char_p))
+                sets[k].n_hotwords = len(words)
+                sets[k].hotword_weight = struct.unpack("<d", wbits)[0]
+            idx_arr = (C.c_int32 * n)(*index)
+            keep_alive += [sets, idx_arr]
+            opts.hot_sets = C.cast(sets, C.POINTER(_lib.HotwordSet))
+            opts.n_hot_sets = len(set_of)
+            opts.utt_hot_set = C.cast(idx_arr, C.POINTER(C.c_int32))
         opts.max_out_beams = int(max_out_beams)
         states_arr = None
         n_lm = len(models)
@@ -378,7 +425,6 @@ class BeamSearchDecoderCTC:
                         raise AssertionError("Wrong input state type found. Expected B200LMState, got %s" % type(part))
                     states_arr[i * n_lm + j] = part._to_c()
             opts.lm_start_states = C.cast(states_arr, C.POINTER(_lib.LMState))
-        keep_alive: List[Any] = []
         if stream is not None:
             opts.stream_states = C.cast(self._stream_states(handle, stream, keep_alive), C.POINTER(_lib.StreamState))
         opts.finalize_mode = int(finalize_mode)
@@ -464,12 +510,19 @@ class BeamSearchDecoderCTC:
                            beam_prune_logp: float = DEFAULT_PRUNE_LOGP, token_min_logp: float = DEFAULT_MIN_TOKEN_LOGP,
                            prune_history: bool = DEFAULT_PRUNE_BEAMS, hotwords: Optional[Iterable[str]] = None,
                            hotword_weight: float = DEFAULT_HOTWORD_WEIGHT,
-                           lengths: Optional[Sequence[int]] = None) -> List[List[OutputBeam]]:
+                           lengths: Optional[Sequence[int]] = None,
+                           hotwords_list: Optional[Sequence[Optional[Iterable[str]]]] = None,
+                           hotword_weight_list: Optional[Sequence[float]] = None) -> List[List[OutputBeam]]:
         """`lengths` (extension, SURVEY 8f-4): valid frames per utterance when `logits_list` is ONE padded
-        [B, T, V] array or (CUDA) tensor -- the padding rows are never read."""
+        [B, T, V] array or (CUDA) tensor -- the padding rows are never read.
+
+        `hotwords_list` / `hotword_weight_list` (extension): one hotword list (or None) and one weight per utterance.
+        Utterance i then gets what ``decode_beams(logits_list[i], hotwords=hotwords_list[i],
+        hotword_weight=hotword_weight_list[i])`` returns, in one batched call."""
         # the reference strips the LM state for multiprocessing (decoder.py:797-799); keep that
         return self._run(logits_list, beam_width, beam_prune_logp, token_min_logp, prune_history, hotwords,
-                         hotword_weight, max_out_beams=beam_width, with_state=False, lengths=lengths)
+                         hotword_weight, max_out_beams=beam_width, with_state=False, lengths=lengths,
+                         hotwords_list=hotwords_list, hotword_weight_list=hotword_weight_list)
 
     def decode(self, logits: Any, beam_width: int = DEFAULT_BEAM_WIDTH, beam_prune_logp: float = DEFAULT_PRUNE_LOGP,
                token_min_logp: float = DEFAULT_MIN_TOKEN_LOGP, hotwords: Optional[Iterable[str]] = None,
@@ -481,9 +534,12 @@ class BeamSearchDecoderCTC:
     def decode_batch(self, pool: Any, logits_list: Sequence[Any], beam_width: int = DEFAULT_BEAM_WIDTH,
                      beam_prune_logp: float = DEFAULT_PRUNE_LOGP, token_min_logp: float = DEFAULT_MIN_TOKEN_LOGP,
                      hotwords: Optional[Iterable[str]] = None, hotword_weight: float = DEFAULT_HOTWORD_WEIGHT,
-                     lengths: Optional[Sequence[int]] = None) -> List[str]:
+                     lengths: Optional[Sequence[int]] = None, hotwords_list: Optional[Sequence[Optional[Iterable[str]]]] = None,
+                     hotword_weight_list: Optional[Sequence[float]] = None) -> List[str]:
+        """`hotwords_list` / `hotword_weight_list` (extension): per-utterance hotwords, as in decode_beams_batch."""
         return self._run(logits_list, beam_width, beam_prune_logp, token_min_logp, True, hotwords, hotword_weight,
-                         max_out_beams=1, with_state=False, texts_only=True, lengths=lengths)
+                         max_out_beams=1, with_state=False, texts_only=True, lengths=lengths,
+                         hotwords_list=hotwords_list, hotword_weight_list=hotword_weight_list)
 
     # ---- streaming (reference decoder.py:669-728) ------------------------------------------------
     def get_starting_state(self) -> Tuple[List[Beam], LMScoreCache, Dict[str, float]]:
@@ -739,11 +795,21 @@ class BeamSearchDecoderCTC:
                                    beam_width: int = DEFAULT_BEAM_WIDTH, beam_prune_logp: float = DEFAULT_PRUNE_LOGP,
                                    token_min_logp: float = DEFAULT_MIN_TOKEN_LOGP, prune_history: bool = DEFAULT_PRUNE_BEAMS,
                                    hotword_scorer: Optional[HotwordScorer] = None, force_next_word: bool = False,
-                                   is_end: bool = False) -> List[List[LMBeam]]:
-        """Extension: many independent streams advance by one chunk each in ONE kernel launch."""
+                                   is_end: bool = False,
+                                   hotword_scorer_list: Optional[Sequence[Optional[HotwordScorer]]] = None) -> List[List[LMBeam]]:
+        """Extension: many independent streams advance by one chunk each in ONE kernel launch.  `hotword_scorer_list`:
+        one HotwordScorer (or None) per stream instead of one `hotword_scorer` for all."""
         n = len(logits_list)
         if not (len(beams_list) == len(processed_frames_list) == len(cached_lm_scores_list) == n):
             raise ValueError("one beam list, cache and processed_frames value per stream")
+        hot_list = weight_list = None
+        if hotword_scorer_list is not None:
+            if hotword_scorer is not None:
+                raise ValueError("pass either hotword_scorer or hotword_scorer_list, not both")
+            if len(hotword_scorer_list) != n:
+                raise ValueError("hotword_scorer_list has %d entries for %d streams" % (len(hotword_scorer_list), n))
+            hot_list = [s.unigrams if s is not None else None for s in hotword_scorer_list]
+            weight_list = [s.weight if s is not None else DEFAULT_HOTWORD_WEIGHT for s in hotword_scorer_list]
         lm = self._language_model
         starts: Optional[List[Optional[AbstractLMState]]] = None
         if lm is not None:
@@ -756,7 +822,8 @@ class BeamSearchDecoderCTC:
         mode = _lib.FIN_EOS if is_end else (_lib.FIN_FLUSH if force_next_word else _lib.FIN_KEEP)
         return self._run(logits_list, beam_width, beam_prune_logp, token_min_logp, prune_history, hot, weight,
                          max_out_beams=beam_width, lm_start_states=starts, with_state=False,
-                         stream=[(list(b), int(p)) for b, p in zip(beams_list, processed_frames_list)], finalize_mode=mode)
+                         stream=[(list(b), int(p)) for b, p in zip(beams_list, processed_frames_list)], finalize_mode=mode,
+                         hotwords_list=hot_list, hotword_weight_list=weight_list)
 
     # ---- serialisation (reference decoder.py:947-1005): file plumbing only ------------------
     def save_to_dir(self, filepath: str) -> None:

@@ -123,11 +123,18 @@ def build_ctcdecoder_broadcast(labels: List[str], kenlm_model_path: Optional[str
 
 def decode_batch_sharded(decoder: BeamSearchDecoderCTC, logits_list: Sequence[Any], group: Any = None, **kwargs: Any) -> List[str]:
     """Every rank passes the SAME list; each decodes its shard on its own GPU; all ranks return the
-    full list of transcripts (one all_gather_object of strings -- not on the data path)."""
+    full list of transcripts (one all_gather_object of strings -- not on the data path).  Per-utterance
+    ``hotwords_list`` / ``hotword_weight_list`` are sharded together with the utterances."""
     import torch.distributed as dist
 
     world, rank = dist.get_world_size(group), dist.get_rank(group)
     shards = shard_utterances([x.shape[0] for x in logits_list], world)
+    for key in ("hotwords_list", "hotword_weight_list"):
+        if kwargs.get(key) is not None:
+            per_utt = list(kwargs[key])
+            if len(per_utt) != len(logits_list):
+                raise ValueError("%s has %d entries for %d utterances" % (key, len(per_utt), len(logits_list)))
+            kwargs[key] = [per_utt[i] for i in shards[rank]]
     mine = decoder.decode_batch(None, [logits_list[i] for i in shards[rank]], **kwargs)
     gathered: List[Any] = [None] * world
     dist.all_gather_object(gathered, mine, group=group)
