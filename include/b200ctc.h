@@ -137,6 +137,15 @@ typedef struct {
     double hotword_weight;
 } b2c_hotword_set_t;
 
+/* One language-model set: no model (n_models == 0), a LanguageModel (1) or a MultiLanguageModel of 2..4 models, each
+ * with its own alpha / beta / unk offset / boundary flag, as b2c_decoder_set_params_lm gives a decoder's own models. */
+typedef struct b2c_lm_set {
+    int n_models;
+    b2c_lm_t* models[4];
+    double alpha[4], beta[4], unk_score_offset[4];
+    int lm_score_boundary[4];
+} b2c_lm_set_t;
+
 typedef struct {
     int beam_width;            /* DEFAULT_BEAM_WIDTH 100          (constants.py:8)  */
     double beam_prune_logp;    /* DEFAULT_PRUNE_LOGP -10          (constants.py:10) */
@@ -161,6 +170,16 @@ typedef struct {
     const b2c_hotword_set_t* hot_sets;
     int n_hot_sets;
     const int32_t* utt_hot_set; /* NULL, or [n_utts] indices into hot_sets */
+    /* per-utterance language models: utterance i is decoded exactly as a call of its own on a decoder created with the
+     * models of lm_sets[utt_lm_set[i]] (and their parameters).  utt_lm_set NULL: every utterance uses the decoder's
+     * own model(s) and lm_sets is not read.  Models are uploaded to the decoder's device on first use.  B2C_E_ARG: an
+     * index outside [0, n_lm_sets), a set with a NULL model or with n_models outside [0, 4], or utt_lm_set together
+     * with lm_start_states or stream_states.  Results: b2c_result_lm_state(_at) return the states of the utterance's
+     * own set (0 for an utterance without a model); in b2c_packed_t n_models is the largest set of the call, and a
+     * beam of a smaller set has its models' states first, then zeroed states (length 0). */
+    const struct b2c_lm_set* lm_sets;
+    int n_lm_sets;
+    const int32_t* utt_lm_set; /* NULL, or [n_utts] indices into lm_sets */
 } b2c_decode_opts_t;
 void b2c_decode_opts_default(b2c_decode_opts_t* opts);
 

@@ -37,6 +37,11 @@ class HotwordSet(C.Structure):
     _fields_ = [("hotwords", C.POINTER(C.c_char_p)), ("n_hotwords", C.c_int), ("hotword_weight", C.c_double)]
 
 
+class LmSet(C.Structure):
+    _fields_ = [("n_models", C.c_int), ("models", C.c_void_p * 4), ("alpha", C.c_double * 4), ("beta", C.c_double * 4),
+                ("unk_score_offset", C.c_double * 4), ("lm_score_boundary", C.c_int * 4)]
+
+
 class DecodeOpts(C.Structure):
     _fields_ = [
         ("beam_width", C.c_int),
@@ -54,6 +59,9 @@ class DecodeOpts(C.Structure):
         ("hot_sets", C.POINTER(HotwordSet)),
         ("n_hot_sets", C.c_int),
         ("utt_hot_set", C.POINTER(C.c_int32)),
+        ("lm_sets", C.POINTER(LmSet)),
+        ("n_lm_sets", C.c_int),
+        ("utt_lm_set", C.POINTER(C.c_int32)),
     ]
 
 

@@ -150,7 +150,7 @@ struct B2cBeamArgs {
     const u32* s_word_len;
     int fin_mode;                    // B2C_FIN_*
     int* out_aux;                    // [n_utts][out_beams][4], streaming calls only
-    B2cLmState* out_states_x;        // [n_utts][out_beams][n_lm - 1], MultiLanguageModel only
+    B2cLmState* out_states_x;        // [n_utts][out_beams][P.lm_x], calls with a MultiLanguageModel only
     // outputs
     int* out_nbeams;
     int* out_status;
@@ -220,7 +220,7 @@ B2C_HD void b2c_beam_block(const B2cBeamArgs& A, int slot, u8* smem) {
             sin.word_len = A.s_word_len;
             t0_frames = su.t0;
         }
-        b2c_utt_begin(A.P, W, u, A.start_states ? A.start_states + static_cast<u64>(u) * (A.P.n_lm > 1 ? A.P.n_lm : 1) : nullptr,
+        b2c_utt_begin(A.P, W, u, A.start_states ? A.start_states + static_cast<u64>(u) * (A.P.lm_x + 1) : nullptr,
                       static_cast<int>(rec.cnt), sin);
 #if defined(__CUDACC__)
 #pragma unroll 1
@@ -268,7 +268,7 @@ B2C_HD void b2c_beam_block(const B2cBeamArgs& A, int slot, u8* smem) {
         O.frames = A.out_frames + 2 * ob * (f0 + static_cast<u64>(u));
         O.states = A.out_states + static_cast<u64>(u) * ob;
         O.aux = A.out_aux ? A.out_aux + 4 * static_cast<u64>(u) * ob : nullptr;
-        O.states_x = A.out_states_x ? A.out_states_x + static_cast<u64>(u) * ob * (A.P.n_lm - 1) : nullptr;
+        O.states_x = A.out_states_x ? A.out_states_x + static_cast<u64>(u) * ob * A.P.lm_x : nullptr;
         b2c_finalize(A.P, W, O, A.fin_mode);
         B2C_MARK(8);
     }
@@ -546,9 +546,11 @@ struct b2c_decoder {
     std::vector<ExtraLm> lmx;
     int n_sm = 1;
     size_t smem_optin = 48 * 1024;
-    DevBuf d_raw, d_lmx, d_stream, d_mstats, d_sumk, d_clk, d_maxk, d_toks, d_logits, d_meta, d_tok_start, d_tok_ids, d_tok_lp, d_rowsum, d_set, d_isprob, d_approx, d_ws, d_hot, d_states,
+    DevBuf d_raw, d_lms, d_stream, d_mstats, d_sumk, d_clk, d_maxk, d_toks, d_logits, d_meta, d_tok_start, d_tok_ids, d_tok_lp, d_rowsum, d_set, d_isprob, d_approx, d_ws, d_hot, d_states,
         d_out_small, d_out_toks, d_out_frames;
     PinBuf h_sumk, h_maxk, h_meta, h_out_small, h_out_toks, h_out_frames, h_mstats;
+    PinBuf h_lms;                         // staging of d_lms (pinned: the copy does not go through a driver bounce buffer)
+    std::vector<u8> lms_on_device;        // what d_lms holds: a call whose language-model sets are the same copies nothing
     Event ev[6];
     Stream cls_stream[2];                 // concurrent launches of a call: the fast class, the general kernel
     Event cls_done[2];
@@ -595,7 +597,8 @@ struct BeamRes {
 };
 struct b2c_result {
     std::vector<std::vector<BeamRes>> utts;
-    bool has_lm = false;
+    bool has_lm = false;       // some utterance has a language model
+    std::vector<int> utt_models;  // [n_utts] models of each utterance's set (0: none)
     std::string joined;        // b2c_result_top_texts: top-1 texts, each followed by '\0'
     bool joined_built = false;
     // b2c_result_packed
@@ -800,7 +803,7 @@ struct OutLayout {
 // opt-in host-side section timing (B200CTC_HOST_PROFILE=1, stderr)
 struct HostProfile {
     std::chrono::steady_clock::time_point t0 = std::chrono::steady_clock::now();
-    double ms[6] = {0, 0, 0, 0, 0, 0};     // [5]: hotword tables (make_hot), a part of [0]
+    double ms[7] = {0, 0, 0, 0, 0, 0, 0};  // [5]: hotword tables (make_hot), [6]: language-model sets (make_lm), parts of [0]
     void mark(int k) { const auto now = std::chrono::steady_clock::now(); ms[k] += std::chrono::duration<double, std::milli>(now - t0).count(); t0 = now; }
 };
 
@@ -822,6 +825,9 @@ struct Call {
     std::vector<B2cHot> hot_tab;      // the tables of the call's sets, back to back
     u64 hot_bytes = 0;
     bool any_hot = false;             // some utterance has hotwords
+    std::vector<u8> lm_blob;          // what d_lms receives: the sets, the [n_utts] set indices, the sets' models 1.. (make_lm)
+    std::vector<int> utt_models;      // [n_utts] models of each utterance's set (0: none)
+    bool any_lm = false;              // some utterance has a language model
     bool contiguous_dev = false;  // device input, every utterance right behind the previous one
     MetaLayout meta;
     OutLayout out;
@@ -1566,45 +1572,114 @@ static int make_hot(b2c_decoder* d, Call& c) {
     return 0;
 }
 
-// kernel parameters, the extra language models of a MultiLanguageModel, the hotword table
+// The language-model sets of a call: one per opts->lm_sets entry, or set 0 = the decoder's own model(s) for every
+// utterance.  d_lms holds the B2cLmSet descriptors, then [n_utts] set indices, then the models 1.. of every set.
+// Models are uploaded to the decoder's device on first use (b2c_lm_upload is idempotent).
+static int make_lm(b2c_decoder* d, Call& c) {
+    const auto t_start = std::chrono::steady_clock::now();
+    const b2c_decode_opts_t* o = c.opts;
+    const int n = c.g.n_utts;
+    struct Model { b2c_lm* lm; double alpha, beta, unk; int score_boundary; };
+    std::vector<std::vector<Model>> models;
+    if (o->utt_lm_set) {
+        if (o->lm_start_states || o->stream_states) return fail(B2C_E_ARG, "opts->utt_lm_set excludes lm_start_states and stream_states");
+        if (o->n_lm_sets < 0 || (o->n_lm_sets > 0 && !o->lm_sets)) return fail(B2C_E_ARG, "null lm_sets");
+        for (int i = 0; i < n; ++i)
+            if (o->utt_lm_set[i] < 0 || o->utt_lm_set[i] >= o->n_lm_sets) return fail(B2C_E_ARG, "utt_lm_set index out of range");
+        for (int k = 0; k < o->n_lm_sets; ++k) {
+            const b2c_lm_set_t& ls = o->lm_sets[k];
+            if (ls.n_models < 0 || ls.n_models > B2C_MAX_LMS) return fail(B2C_E_ARG, "a language-model set holds 0 to 4 models");
+            std::vector<Model> ms;
+            for (int j = 0; j < ls.n_models; ++j) {
+                if (!ls.models[j]) return fail(B2C_E_ARG, "null model in a language-model set");
+                ms.push_back(Model{ls.models[j], ls.alpha[j], ls.beta[j], ls.unk_score_offset[j], ls.lm_score_boundary[j] ? 1 : 0});
+            }
+            models.push_back(ms);
+        }
+    } else {
+        std::vector<Model> ms;
+        if (d->lm) {
+            ms.push_back(Model{d->lm, d->alpha, d->beta, d->unk, d->score_boundary});
+            for (const b2c_decoder::ExtraLm& x : d->lmx) ms.push_back(Model{x.lm, x.alpha, x.beta, x.unk, x.score_boundary});
+        }
+        models.push_back(ms);
+    }
+    const int n_sets = static_cast<int>(models.size());
+    std::vector<char> used(static_cast<size_t>(n_sets), o->utt_lm_set ? 0 : 1);
+    for (int i = 0; o->utt_lm_set && i < n; ++i) used[o->utt_lm_set[i]] = 1;
+    std::vector<B2cLmSet> sets(static_cast<size_t>(std::max(n_sets, 1)));
+    std::vector<B2cLmExtra> extra;
+    std::vector<size_t> x_off(static_cast<size_t>(n_sets), 0);
+    int max_models = 0;
+    for (int k = 0; k < n_sets; ++k) {
+        B2cLmSet& M = sets[k];
+        std::memset(&M, 0, sizeof(M));
+        M.log_base_change = 0x1.26bb1bbb55516p+1;  // 1.0 / math.log10(math.e) (constants.py:18)
+        M.hist_n = 1;
+        if (!used[k] || models[k].empty()) continue;
+        int max_order = 0;      // MultiLanguageModel.order is the maximum (language_model.py:468-470)
+        x_off[k] = extra.size();
+        for (size_t j = 0; j < models[k].size(); ++j) {
+            const Model& m = models[k][j];
+            B2C_TRY(b2c_lm_upload(m.lm, d->device));
+            const void* blob;
+            {
+                std::lock_guard<std::mutex> lk(m.lm->mu);
+                blob = m.lm->dev.at(d->device);
+            }
+            const B2cLmView v = m.lm->host.view(blob);
+            if (v.order > B2C_MAX_ORDER) return fail(B2C_E_ARG, "n-gram order too large");
+            max_order = std::max(max_order, v.order);
+            if (j == 0) {
+                M.lm = v; M.alpha = m.alpha; M.beta = m.beta; M.unk_offset = m.unk; M.score_boundary = m.score_boundary;
+            } else {
+                B2cLmExtra X;
+                std::memset(&X, 0, sizeof(X));
+                X.lm = v; X.alpha = m.alpha; X.beta = m.beta; X.unk_offset = m.unk; X.score_boundary = m.score_boundary;
+                extra.push_back(X);
+            }
+        }
+        M.n_lm = static_cast<int>(models[k].size());
+        M.hist_n = std::max(1, max_order - 1);
+        max_models = std::max(max_models, M.n_lm);
+    }
+    const u64 sets_bytes = al16(sizeof(B2cLmSet) * sets.size()), idx_bytes = al16(4ull * static_cast<u64>(std::max(n, 1)));
+    c.lm_blob.assign(sets_bytes + idx_bytes + sizeof(B2cLmExtra) * extra.size(), 0);
+    const void* before = d->d_lms.p;
+    if (d->d_lms.ensure(c.lm_blob.size())) return B2C_E_NOMEM;
+    if (d->d_lms.p != before) d->lms_on_device.clear();   // a new buffer holds nothing yet
+    u8* dev = d->d_lms.as<u8>();
+    for (int k = 0; k < n_sets; ++k)
+        if (sets[k].n_lm > 1) sets[k].lmx = reinterpret_cast<const B2cLmExtra*>(dev + sets_bytes + idx_bytes) + x_off[k];
+    std::memcpy(c.lm_blob.data(), sets.data(), sizeof(B2cLmSet) * sets.size());
+    u32* idx = reinterpret_cast<u32*>(c.lm_blob.data() + sets_bytes);
+    c.utt_models.resize(static_cast<size_t>(n));
+    c.any_lm = false;
+    for (int i = 0; i < n; ++i) {
+        idx[i] = o->utt_lm_set ? static_cast<u32>(o->utt_lm_set[i]) : 0u;
+        c.utt_models[i] = sets[idx[i]].n_lm;
+        c.any_lm = c.any_lm || sets[idx[i]].n_lm > 0;
+    }
+    if (!extra.empty()) std::memcpy(c.lm_blob.data() + sets_bytes + idx_bytes, extra.data(), sizeof(B2cLmExtra) * extra.size());
+    c.P.lm_sets = reinterpret_cast<const B2cLmSet*>(dev);
+    c.P.utt_lm = reinterpret_cast<const u32*>(dev + sets_bytes);
+    c.P.lm_x = std::max(0, max_models - 1);
+    c.g.n_lm = std::max(1, max_models);
+    c.hp.ms[6] += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_start).count();
+    return 0;
+}
+
+// kernel parameters, the language-model sets, the hotword sets
 static int make_params(b2c_decoder* d, Call& c) {
     const b2c_decode_opts_t* o = c.opts;
     B2cParams& P = c.P;
     P.V = c.g.V; P.is_bpe = d->is_bpe; P.has_dup_labels = d->has_dup_labels;
     P.beam_width = o->beam_width; P.prune_history = o->prune_history ? 1 : 0; P.out_beams = c.OB; P.narrow_chain = c.text_only ? 1 : 0;
     P.prune_logp = o->beam_prune_logp; P.token_min_logp = o->token_min_logp;
-    P.alpha = d->alpha; P.beta = d->beta; P.unk_offset = d->unk;
-    P.log_base_change = 0x1.26bb1bbb55516p+1;  // 1.0 / math.log10(math.e) (constants.py:18)
-    P.score_boundary = d->score_boundary; P.bucket_scale = b2c_bucket_scale(o->beam_prune_logp);
+    P.bucket_scale = b2c_bucket_scale(o->beam_prune_logp);
     P.kflags = c.k.no_single ? B2C_FL_NO_SINGLE : 0;
     P.toks = d->d_toks.as<B2cTok>();
-    if (d->lm) {
-        auto it = d->lm->dev.find(d->device);
-        if (it == d->lm->dev.end()) return fail(B2C_E_INTERNAL, "language model is not resident on this device");
-        P.lm = d->lm->host.view(it->second);
-        if (P.lm.order > B2C_MAX_ORDER) return fail(B2C_E_ARG, "n-gram order too large");
-        P.n_lm = 1 + static_cast<int>(d->lmx.size());
-    }
-    int max_order = P.lm.order;     // MultiLanguageModel.order is the maximum (language_model.py:468-470)
-    std::vector<B2cLmExtra> lmx_host(d->lmx.size());
-    for (size_t j = 0; j < d->lmx.size(); ++j) {
-        const b2c_decoder::ExtraLm& x = d->lmx[j];
-        auto it = x.lm->dev.find(d->device);
-        if (it == x.lm->dev.end()) return fail(B2C_E_INTERNAL, "language model is not resident on this device");
-        B2cLmExtra& X = lmx_host[j];
-        std::memset(&X, 0, sizeof(X));
-        X.lm = x.lm->host.view(it->second);
-        if (X.lm.order > B2C_MAX_ORDER) return fail(B2C_E_ARG, "n-gram order too large");
-        X.alpha = x.alpha; X.beta = x.beta; X.unk_offset = x.unk; X.score_boundary = x.score_boundary;
-        max_order = std::max(max_order, X.lm.order);
-    }
-    if (!lmx_host.empty()) {
-        if (d->d_lmx.ensure(sizeof(B2cLmExtra) * lmx_host.size())) return B2C_E_NOMEM;
-        CUDA_OK(cudaMemcpy(d->d_lmx.p, lmx_host.data(), sizeof(B2cLmExtra) * lmx_host.size(), cudaMemcpyHostToDevice));
-        P.lmx = d->d_lmx.as<B2cLmExtra>();
-    }
-    c.g.n_lm = std::max(1, P.n_lm);
-    P.hist_n = std::max(1, max_order - 1);
+    B2C_TRY(make_lm(d, c));
     return make_hot(d, c);
 }
 
@@ -1657,7 +1732,7 @@ static int size_buffers(b2c_decoder* d, Call& c) {
 // call that turns out to hold probabilities is redone as a plain call (B2C_E_RETRY_PLAIN).
 static int choose_pipelined(b2c_decoder* d, Call& c) {
     Geometry& g = c.g;
-    g.hint_ok = d->hint_valid && d->hint_beam == g.beam_width && d->hint_lm == (c.P.lm.order > 0 ? 1 : 0) &&
+    g.hint_ok = d->hint_valid && d->hint_beam == g.beam_width && d->hint_lm == (c.any_lm ? 1 : 0) &&
                 d->hint_hot == (c.any_hot ? 1 : 0) && d->hint_prune == c.P.prune_history && d->hint_frames > 0;
     bool pipe = c.allow_pipe && !c.k.no_pipe && !c.is_device && !c.half_in && g.T_max >= 8 * B2C_TILE_ROWS &&
                 !g.streaming && g.n_lm == 1 && g.beam_width <= 128 && g.hint_ok && !d->pipe_refused;
@@ -1723,6 +1798,13 @@ static int upload(b2c_decoder* d, Call& c) {
     if (!c.hot_tab.empty())
         CUDA_OK(cudaMemcpyAsync(d->d_hot.as<u8>() + (c.hot_bytes - sizeof(B2cHot) * c.hot_tab.size()), c.hot_tab.data(),
                                 sizeof(B2cHot) * c.hot_tab.size(), cudaMemcpyHostToDevice, st));
+    if (c.lm_blob != d->lms_on_device) {   // the same sets as the previous call (e.g. the decoder's own model): already there
+        if (d->h_lms.ensure(c.lm_blob.size())) return B2C_E_NOMEM;
+        std::memcpy(d->h_lms.p, c.lm_blob.data(), c.lm_blob.size());
+        d->lms_on_device.clear();          // until the copy is enqueued
+        CUDA_OK(cudaMemcpyAsync(d->d_lms.p, d->h_lms.p, c.lm_blob.size(), cudaMemcpyHostToDevice, st));
+        d->lms_on_device = c.lm_blob;
+    }
     if (c.opts->lm_start_states) {
         // with a MultiLanguageModel: n_lm consecutive states per utterance (MultiLanguageModelState.states)
         std::vector<B2cLmState> start_host(static_cast<size_t>(n) * c.g.n_lm);
@@ -1990,7 +2072,7 @@ static int read_back(b2c_decoder* d, Call& c) {
     d->tm.d2h_bytes += static_cast<long long>(c.out.bytes + c.tok_bytes + (c.text_only ? 0 : c.frm_bytes) + 8ull * n + 32);
     const u32* ms = d->h_mstats.as<u32>();
     d->hint_valid = true;
-    d->hint_beam = c.opts->beam_width; d->hint_lm = c.P.lm.order > 0 ? 1 : 0; d->hint_hot = c.any_hot ? 1 : 0; d->hint_prune = c.P.prune_history;
+    d->hint_beam = c.opts->beam_width; d->hint_lm = c.any_lm ? 1 : 0; d->hint_hot = c.any_hot ? 1 : 0; d->hint_prune = c.P.prune_history;
     for (int q = 0; q < 6; ++q) d->hint_over[q] = ms[q];
     d->hint_frames = ms[6];
     for (int q = 0; q < 7; ++q) d->tm.cand_hist[q] = ms[q];
@@ -2104,7 +2186,8 @@ static void assemble_range(const b2c_decoder* d, const Call& c, b2c_result* res,
             br.logit = h.scores[2 * k];
             br.lm = h.scores[2 * k + 1];
             br.st = h.states[k];
-            if (h.states_x) br.stx.assign(h.states_x + k * (n_lm - 1), h.states_x + (k + 1) * (n_lm - 1));
+            if (h.states_x && c.utt_models[u] > 1)
+                br.stx.assign(h.states_x + k * (n_lm - 1), h.states_x + k * (n_lm - 1) + (c.utt_models[u] - 1));
             if (c.text_only) assemble_text(d, h_toks + base + r * stride, h.ntok[k], br);
             else assemble_beam(d, h_toks + base + r * stride, h.ntok[k], h_frames + 2 * (base + r * stride), h.nwords[k], br);
             if (h.aux) {
@@ -2169,6 +2252,8 @@ static int decode_batch_locked(b2c_decoder_t* d, const void* const* logits, cons
     B2C_TRY(set_geometry(c));
     B2C_TRY(flatten_stream_states(d, c));
     B2C_TRY(make_params(d, c));
+    res->has_lm = c.any_lm;
+    res->utt_models = c.utt_models;
     B2C_TRY(size_buffers(d, c));
     B2C_TRY(choose_pipelined(d, c));
     B2C_TRY(upload(d, c));
@@ -2183,8 +2268,8 @@ static int decode_batch_locked(b2c_decoder_t* d, const void* const* logits, cons
     assemble(d, c, res.get());
     c.hp.mark(4);                                 // statistics read-back, result assembly
     if (c.k.host_prof)
-        std::fprintf(stderr, "[b2c host ms] enqueue=%.3f wait_prepare=%.3f plan=%.3f wait_beam=%.3f assemble=%.3f hotwords=%.3f\n",
-                     c.hp.ms[0], c.hp.ms[1], c.hp.ms[2], c.hp.ms[3], c.hp.ms[4], c.hp.ms[5]);
+        std::fprintf(stderr, "[b2c host ms] enqueue=%.3f wait_prepare=%.3f plan=%.3f wait_beam=%.3f assemble=%.3f hotwords=%.3f lm_sets=%.3f\n",
+                     c.hp.ms[0], c.hp.ms[1], c.hp.ms[2], c.hp.ms[3], c.hp.ms[4], c.hp.ms[5], c.hp.ms[6]);
     *out = res.release();
     return 0;
 }
@@ -2242,9 +2327,11 @@ int b2c_result_packed(b2c_result_t* r, b2c_packed_t* out) {
                 r->pk_frames.insert(r->pk_frames.end(), b.frames.begin(), b.frames.end());
                 r->pk_texts += b.text;
                 r->pk_texts.push_back('\0');
-                for (int j = 0; j < nm; ++j) {
+                for (int j = 0; j < nm; ++j) {     // a smaller set than the call's largest: zeroed states behind its own
                     b2c_lm_state_t st;
-                    from_internal(j == 0 ? b.st : b.stx[static_cast<size_t>(j) - 1], &st);
+                    std::memset(&st, 0, sizeof(st));
+                    if (j == 0) from_internal(b.st, &st);
+                    else if (static_cast<size_t>(j) <= b.stx.size()) from_internal(b.stx[static_cast<size_t>(j) - 1], &st);
                     r->pk_states.push_back(st);
                 }
                 if (r->streaming) {
@@ -2286,12 +2373,12 @@ int b2c_result_n_words(const b2c_result_t* r, int u, int b) { return static_cast
 const char* b2c_result_word(const b2c_result_t* r, int u, int b, int w) { return r->utts[u][b].words[w].c_str(); }
 const int32_t* b2c_result_frames(const b2c_result_t* r, int u, int b) { return r->utts[u][b].frames.data(); }
 int b2c_result_lm_state(const b2c_result_t* r, int u, int b, b2c_lm_state_t* out) {
-    if (!r->has_lm) return 0;
+    if (!r->has_lm || r->utt_models[u] == 0) return 0;
     from_internal(r->utts[u][b].st, out);
     return 1;
 }
 int b2c_result_lm_state_at(const b2c_result_t* r, int u, int b, int lm_index, b2c_lm_state_t* out) {
-    if (!r->has_lm) return 0;
+    if (!r->has_lm || r->utt_models[u] == 0) return 0;
     const BeamRes& br = r->utts[u][b];
     if (lm_index == 0) { from_internal(br.st, out); return 1; }
     if (lm_index < 0 || lm_index > static_cast<int>(br.stx.size())) return 0;

@@ -61,7 +61,10 @@ struct B2cScalars {
     u32 inplace_bad;     // a thread's exactness check of b2c_inplace_step failed (rare)
     u32 m_inplace;       // frames handled by b2c_inplace_step
     u32 clean_s, clean_g; // leading slots of the shared-memory / HBM tier's grouping table that are known to be clear
+    u32 lm_set;          // this utterance's language-model set, an index into B2cParams::lm_sets (b2c_utt_begin)
 };
+// the language-model set of the CTA's current utterance
+B2C_HD const B2cLmSet& b2c_lm_of(const B2cParams& P, const B2cScalars* sc) { return P.lm_sets[sc->lm_set]; }
 enum { B2C_FL_BPE = 1, B2C_FL_PRUNE = 2, B2C_FL_LM = 4, B2C_FL_PSCORE = 8, B2C_FL_NO_SINGLE = 16 };
 
 #define B2C_NBUCKET 256      // score buckets of the O(m) ranking (monotone in the score)
@@ -252,29 +255,29 @@ B2C_HD B2cLmState* b2c_text_states_x(const B2cText* arena, u32 text_cap, int n_l
     return reinterpret_cast<B2cLmState*>(const_cast<B2cText*>(arena) + text_cap) + static_cast<u64>(node) * static_cast<u64>(n_lm - 1);
 }
 // out_x: where the end states of models 1.. go (MultiLanguageModel; nullptr: not wanted)
-B2C_HDN void b2c_text_extend(B2cParams P, const B2cHotSet& H, const B2cText* arena, u32 text_cap, u32 parent_id, u64 word_hash,
+B2C_HDN void b2c_text_extend(const B2cLmSet& M, const B2cHotSet& H, const B2cText* arena, u32 text_cap, u32 parent_id, u64 word_hash,
                              u32 word_len, int is_eos, B2cTextNew* out, B2cLmState* out_x) {
     const B2cText* parent = arena + parent_id;
     out->hw_count = parent->hw_count + b2c_hot_is_word(H, word_hash, word_len);
-    if (P.n_lm > 1) {
+    if (M.n_lm > 1) {
         // MultiLanguageModel.score (language_model.py:485-502): sum of the models' scores, left to right, / N
-        const B2cLmState* px = b2c_text_states_x(arena, text_cap, P.n_lm, parent_id);
+        const B2cLmState* px = b2c_text_states_x(arena, text_cap, M.n_lm, parent_id);
         B2cLmState in = parent->st;
-        double sc = b2c_lm_score_word(P, in, word_hash, word_len, is_eos != 0, out->st);
-        for (int j = 1; j < P.n_lm; ++j) {
-            const B2cLmExtra X = P.lmx[j - 1];
+        double sc = b2c_lm_score_word(M, in, word_hash, word_len, is_eos != 0, out->st);
+        for (int j = 1; j < M.n_lm; ++j) {
+            const B2cLmExtra X = M.lmx[j - 1];
             in = px[j - 1];
             B2cLmState end;
-            sc = sc + b2c_lm_score_word_v(X.lm, X.alpha, X.beta, X.unk_offset, X.score_boundary, P.log_base_change, in, word_hash,
+            sc = sc + b2c_lm_score_word_v(X.lm, X.alpha, X.beta, X.unk_offset, X.score_boundary, M.log_base_change, in, word_hash,
                                           word_len, is_eos != 0, end);
             if (out_x) out_x[j - 1] = end;
         }
-        sc = sc / static_cast<double>(P.n_lm);
+        sc = sc / static_cast<double>(M.n_lm);
         out->raw_lm = parent->raw_lm + sc;
         out->lm_hw = out->raw_lm + H.weight * static_cast<double>(out->hw_count);
-    } else if (P.lm.order > 0) {
+    } else if (M.lm.order > 0) {
         B2cLmState in = parent->st;
-        double sc = b2c_lm_score_word(P, in, word_hash, word_len, is_eos != 0, out->st);
+        double sc = b2c_lm_score_word(M, in, word_hash, word_len, is_eos != 0, out->st);
         out->raw_lm = parent->raw_lm + sc;
         out->lm_hw = out->raw_lm + H.weight * static_cast<double>(out->hw_count);
     } else {
@@ -310,23 +313,23 @@ B2C_HDN double b2c_partial_score_ool(const B2cHotSet& H, int lm_order, int have_
 }
 // MultiLanguageModel.score_partial_token (language_model.py:478-483): mean over the models; the hotword prefix
 // score takes precedence exactly as with one model (decoder.py:397-409)
-B2C_HDN double b2c_partial_score_multi(B2cParams P, const B2cHotSet& H, u64 part_hash, u32 part_len) {
+B2C_HDN double b2c_partial_score_multi(const B2cLmSet& M, const B2cHotSet& H, u64 part_hash, u32 part_len) {
     if (H.min_len > 0) {
         if (part_len == 0) return H.weight * 0 / H.min_len;
         const B2cHot* h = b2c_hot_find(H, part_hash);
         if (h) return H.weight * static_cast<double>(part_len) / static_cast<double>(h->min_len);
     }
-    double s = b2c_lm_partial_v(P.lm, P.unk_offset, part_hash, part_len);
-    for (int j = 1; j < P.n_lm; ++j) {
-        const B2cLmExtra X = P.lmx[j - 1];
+    double s = b2c_lm_partial_v(M.lm, M.unk_offset, part_hash, part_len);
+    for (int j = 1; j < M.n_lm; ++j) {
+        const B2cLmExtra X = M.lmx[j - 1];
         s = s + b2c_lm_partial_v(X.lm, X.unk_offset, part_hash, part_len);
     }
-    return s / static_cast<double>(P.n_lm);
+    return s / static_cast<double>(M.n_lm);
 }
-B2C_HD double b2c_partial_score_of(const B2cParams& P, const B2cHotSet& H, bool need, u64 part_hash, u32 part_len) {
+B2C_HD double b2c_partial_score_of(const B2cLmSet& M, const B2cHotSet& H, bool need, u64 part_hash, u32 part_len) {
     if (!need) return 0.0;
-    if (P.n_lm > 1) return b2c_partial_score_multi(P, H, part_hash, part_len);
-    return b2c_partial_score_ool(H, P.lm.order, P.lm.have_unigrams, P.lm.prefixes, P.lm.prefix_mask, P.unk_offset, part_hash, part_len);
+    if (M.n_lm > 1) return b2c_partial_score_multi(M, H, part_hash, part_len);
+    return b2c_partial_score_ool(H, M.lm.order, M.lm.have_unigrams, M.lm.prefixes, M.lm.prefix_mask, M.unk_offset, part_hash, part_len);
 }
 
 // history-prune hash of "text + word" (last hist_n words)
@@ -339,17 +342,17 @@ B2C_HDN u64 b2c_hist_extend(const B2cText* par, int hist_n, u64 word_hash) {
 
 // a surviving beam finished a word: create the text node (LM state, raw score, hotword count, history)
 struct B2cTextCommit { u32 node; double lm_hw; u64 hist_hash; };
-B2C_HDN void b2c_commit_text(B2cParams P, const B2cHotSet& H, B2cText* arena, u32 text_cap, u32* text_used, u32* status, u32 parent_id,
+B2C_HDN void b2c_commit_text(const B2cLmSet& M, const B2cHotSet& H, B2cText* arena, u32 text_cap, u32* text_used, u32* status, u32 parent_id,
                              u64 word_hash, u32 word_len, B2cTextCommit* out) {
     const B2cText* par = arena + parent_id;
     // the node is allocated first so that a MultiLanguageModel's other end states are written in place
     const u32 id = b2c_atomic_add_u32(text_used, 1u);
     B2cTextNew tn;
-    b2c_text_extend(P, H, arena, text_cap, parent_id, word_hash, word_len, 0, &tn,
-                    (P.n_lm > 1 && id < text_cap) ? b2c_text_states_x(arena, text_cap, P.n_lm, id) : nullptr);
+    b2c_text_extend(M, H, arena, text_cap, parent_id, word_hash, word_len, 0, &tn,
+                    (M.n_lm > 1 && id < text_cap) ? b2c_text_states_x(arena, text_cap, M.n_lm, id) : nullptr);
     out->lm_hw = tn.lm_hw;
     out->node = parent_id;
-    const u32 keep = (par->n_win + 1 < static_cast<u32>(P.hist_n)) ? par->n_win : static_cast<u32>(P.hist_n) - 1;
+    const u32 keep = (par->n_win + 1 < static_cast<u32>(M.hist_n)) ? par->n_win : static_cast<u32>(M.hist_n) - 1;
     B2cText nt;
     nt.win[0] = word_hash;
     for (u32 w = 0; w < keep; ++w) nt.win[w + 1] = par->win[w];
@@ -685,7 +688,7 @@ B2C_HD void b2c_commit_one(const B2cParams& P, const B2cWork& W, const Tier& C, 
     u64 hh = cur.hist_hash[bl];
     if (word_len > 0) {
         B2cTextCommit tc;
-        b2c_commit_text(P, sc->hot, W.text, W.text_cap, &sc->text_used, &sc->status, tnode, cur.part_hash[bl], word_len, &tc);
+        b2c_commit_text(b2c_lm_of(P, sc), sc->hot, W.text, W.text_cap, &sc->text_used, &sc->status, tnode, cur.part_hash[bl], word_len, &tc);
         tnode = tc.node;
         lm_hw = tc.lm_hw;
         hh = tc.hist_hash;
@@ -695,7 +698,7 @@ B2C_HD void b2c_commit_one(const B2cParams& P, const B2cWork& W, const Tier& C, 
     nx.hist_hash[j] = hh;
     double ps = 0.0;
     if (type == 0) ps = cur.pscore[bl];
-    else if (part_len > 0) ps = b2c_partial_score_of(P, sc->hot, (flags & B2C_FL_PSCORE) != 0, part_hash, part_len);
+    else if (part_len > 0) ps = b2c_partial_score_of(b2c_lm_of(P, sc), sc->hot, (flags & B2C_FL_PSCORE) != 0, part_hash, part_len);
     nx.pscore[j] = ps;
 }
 
@@ -821,12 +824,12 @@ B2C_HD void b2c_frame_step(const B2cParams& P, B2cWork& W, int t, const u32* tk_
             double lm_hw = cur.lm_hw[bl];
             if ((type == 1 || type == 2) && cur.part_len[bl] > 0) {
                 B2cTextNew tn;
-                b2c_text_extend(P, sc->hot, W.text, W.text_cap, cur.text_node[bl], cur.part_hash[bl], cur.part_len[bl], 0, &tn, nullptr);
+                b2c_text_extend(b2c_lm_of(P, sc), sc->hot, W.text, W.text_cap, cur.text_node[bl], cur.part_hash[bl], cur.part_len[bl], 0, &tn, nullptr);
                 lm_hw = tn.lm_hw;
             }
             double ps = 0.0;
             if (type == 0) ps = cur.pscore[bl];
-            else if (part_len > 0) ps = b2c_partial_score_of(P, sc->hot, (flags & B2C_FL_PSCORE) != 0, cph & B2C_PH_MASK, part_len);
+            else if (part_len > 0) ps = b2c_partial_score_of(b2c_lm_of(P, sc), sc->hot, (flags & B2C_FL_PSCORE) != 0, cph & B2C_PH_MASK, part_len);
             const double sco = b2c_combine_score((flags & B2C_FL_LM) != 0, s, lm_hw, ps, part_len);
             const u64 key = b2c_f64_key(sco);
             C.ckey[i] = key;
@@ -881,7 +884,7 @@ B2C_HD void b2c_frame_step(const B2cParams& P, B2cWork& W, int t, const u32* tk_
                 const u32 meta = C.cmeta[last];
                 u64 hh = cur.hist_hash[bl];
                 if ((type == 1 || type == 2) && cur.part_len[bl] > 0)
-                    hh = b2c_hist_extend(W.text + cur.text_node[bl], P.hist_n, cur.part_hash[bl]);
+                    hh = b2c_hist_extend(W.text + cur.text_node[bl], b2c_lm_of(P, sc).hist_n, cur.part_hash[bl]);
                 const u64 hk = b2c_beam_key(hh, cph & B2C_PH_MASK, meta & 0xFFFFu, meta >> 16);
                 phk[rank] = hk;
                 b2c_fence_block();
@@ -964,7 +967,7 @@ B2C_HD bool b2c_inplace_step(const B2cParams& P, const B2cWork& W, int t, int ki
         B2C_FOR(b, n) {
             const u64 nph = b2c_hash_append(cur.part_hash[b], ti.raw_hash, ti.raw_pow);
             const u32 nplen = (static_cast<u32>(cur.part_len[b]) + ti.raw_nchars) & 0xFFFFu;
-            const double ps = b2c_partial_score_of(P, sc->hot, true, nph, nplen);
+            const double ps = b2c_partial_score_of(b2c_lm_of(P, sc), sc->hot, true, nph, nplen);
             union { double d; u64 u; } c;
             c.d = ps;
             Cs.ckey[b] = c.u;
@@ -1093,11 +1096,13 @@ B2C_HDN void b2c_utt_begin(B2cParams P, B2cWork W, int u, const B2cLmState* star
         sc->inplace_bad = 0;
         sc->prev_max = 0.0;
         sc->hot = P.hot_utt[u];
+        sc->lm_set = P.utt_lm[u];
+        const B2cLmSet& M = P.lm_sets[sc->lm_set];
         u32 fl = 0;
         if (P.is_bpe) fl |= B2C_FL_BPE;
         if (P.prune_history) fl |= B2C_FL_PRUNE;
-        if (P.lm.order > 0) fl |= B2C_FL_LM;
-        if (sc->hot.min_len > 0 || P.lm.order > 0) fl |= B2C_FL_PSCORE;
+        if (M.lm.order > 0) fl |= B2C_FL_LM;
+        if (sc->hot.min_len > 0 || M.lm.order > 0) fl |= B2C_FL_PSCORE;
         fl |= static_cast<u32>(P.kflags) & B2C_FL_NO_SINGLE;
         sc->flags = fl;
         B2cText root;
@@ -1107,35 +1112,35 @@ B2C_HDN void b2c_utt_begin(B2cParams P, B2cWork W, int u, const B2cLmState* star
         root.raw_lm = 0.0;
         root.hw_count = 0;
         root.st.length = 0;
-        if (P.lm.order > 0) {
+        if (M.lm.order > 0) {
             if (start_state) {
                 root.st = *start_state;
-            } else if (P.score_boundary) {   // BeginSentenceWrite (language_model.py:311-312)
+            } else if (M.score_boundary) {   // BeginSentenceWrite (language_model.py:311-312)
                 root.st.length = 1;
-                root.st.words[0] = P.lm.bos_id;
-                root.st.backoff[0] = P.lm.uni[P.lm.bos_id].backoff;
+                root.st.words[0] = M.lm.bos_id;
+                root.st.backoff[0] = M.lm.uni[M.lm.bos_id].backoff;
             }
         }
         W.text[0] = root;
-        if (P.n_lm > 1) {       // start states of models 1.. (start_state, if given, holds n_lm consecutive states)
-            B2cLmState* x = b2c_text_states_x(W.text, W.text_cap, P.n_lm, 0);
-            for (int j = 1; j < P.n_lm; ++j) {
+        if (M.n_lm > 1) {       // start states of models 1.. (start_state, if given, holds n_lm consecutive states)
+            B2cLmState* x = b2c_text_states_x(W.text, W.text_cap, M.n_lm, 0);
+            for (int j = 1; j < M.n_lm; ++j) {
                 B2cLmState st;
                 st.length = 0;
                 for (int w = 0; w < B2C_MAX_HIST; ++w) { st.words[w] = 0; st.backoff[w] = 0.0f; }
                 if (start_state) {
                     st = start_state[j];
-                } else if (P.lmx[j - 1].score_boundary) {
+                } else if (M.lmx[j - 1].score_boundary) {
                     st.length = 1;
-                    st.words[0] = P.lmx[j - 1].lm.bos_id;
-                    st.backoff[0] = P.lmx[j - 1].lm.uni[P.lmx[j - 1].lm.bos_id].backoff;
+                    st.words[0] = M.lmx[j - 1].lm.bos_id;
+                    st.backoff[0] = M.lmx[j - 1].lm.uni[M.lmx[j - 1].lm.bos_id].backoff;
                 }
                 x[j - 1] = st;
             }
         }
         const B2cBeamTab& c = W.cur;
         c.logit[0] = 0.0;
-        c.lm_hw[0] = P.lm.order > 0 ? 0.0 : sc->hot.weight * 0;
+        c.lm_hw[0] = M.lm.order > 0 ? 0.0 : sc->hot.weight * 0;
         c.pscore[0] = 0.0;
         c.text_hash[0] = B2C_TEXT_SEED;
         c.part_hash[0] = 0;
@@ -1160,11 +1165,12 @@ B2C_HDN void b2c_utt_begin(B2cParams P, B2cWork W, int u, const B2cLmState* star
         const B2cStreamBeam sb = in.beams[b];
         u64 th = B2C_TEXT_SEED, hh = B2C_HIST_SEED;
         u32 node = 0;
-        double lm_hw = P.lm.order > 0 ? 0.0 : sc->hot.weight * 0;
+        const B2cLmSet& M = b2c_lm_of(P, sc);
+        double lm_hw = M.lm.order > 0 ? 0.0 : sc->hot.weight * 0;
         for (u32 w = 0; w < sb.n_words; ++w) {
             const u64 wh = in.word_hash[sb.word_off + w];
             B2cTextCommit tc;
-            b2c_commit_text(P, sc->hot, W.text, W.text_cap, &sc->text_used, &sc->status, node, wh, in.word_len[sb.word_off + w], &tc);
+            b2c_commit_text(M, sc->hot, W.text, W.text_cap, &sc->text_used, &sc->status, node, wh, in.word_len[sb.word_off + w], &tc);
             node = tc.node;
             lm_hw = tc.lm_hw;
             hh = tc.hist_hash;
@@ -1173,7 +1179,7 @@ B2C_HDN void b2c_utt_begin(B2cParams P, B2cWork W, int u, const B2cLmState* star
         const B2cBeamTab& c = W.cur;
         c.logit[b] = sb.logit;
         c.lm_hw[b] = lm_hw;
-        c.pscore[b] = sb.part_len > 0 ? b2c_partial_score_of(P, sc->hot, (sc->flags & B2C_FL_PSCORE) != 0, sb.part_hash, sb.part_len) : 0.0;
+        c.pscore[b] = sb.part_len > 0 ? b2c_partial_score_of(M, sc->hot, (sc->flags & B2C_FL_PSCORE) != 0, sb.part_hash, sb.part_len) : 0.0;
         c.text_hash[b] = th;
         c.part_hash[b] = sb.part_hash;
         c.hist_hash[b] = hh;
@@ -1208,7 +1214,8 @@ struct B2cOut {              // per-utterance output views (HBM)
     u32* toks;               // [out_beams][stride]  token | kind << 16, last emission first
     int* frames;             // [out_beams][stride][2] word frames, last word first
     B2cLmState* states;      // [out_beams] LM state after the last word (last_lm_state)
-    B2cLmState* states_x;    // [out_beams][n_lm - 1] MultiLanguageModel: the other models' states (nullptr otherwise)
+    B2cLmState* states_x;    // [out_beams][P.lm_x] MultiLanguageModel: the other models' states, the first n_lm - 1 of
+                             // each beam's row (nullptr when no set of the call has more than one model)
     int* aux;                // [out_beams][4] streaming: input beam the output descends from (-1: none), canonical
                              // token of last_char (-1: None), partial_frames; nullptr outside streaming calls
     u32 stride;              // T + 1
@@ -1219,6 +1226,7 @@ B2C_HDN void b2c_finalize(B2cParams P, B2cWork W, B2cOut O, int fin_mode) {
     const int is_eos = fin_mode == B2C_FIN_EOS ? 1 : 0;
     // on entry the grouping table is clear for ht_size(n_beams) slots (last phase D / utt_begin)
     B2cScalars* sc = W.sc;
+    const B2cLmSet& M = b2c_lm_of(P, sc);
     const u32 n = sc->n_beams;
     const B2cCandTier C = b2c_pick_tier(W, n);
     const u32 hmask = b2c_ht_size(n) - 1;
@@ -1248,16 +1256,16 @@ B2C_HDN void b2c_finalize(B2cParams P, B2cWork W, B2cOut O, int fin_mode) {
         double lm_hw;
         if (keep) {
             lm_hw = cur.lm_hw[last];        // next_word == "": cache hit on (text, False) (decoder.py:387-396)
-        } else if ((P.lm.order > 0 && (is_eos || cur.part_len[last] > 0)) || cur.part_len[last] > 0) {
+        } else if ((M.lm.order > 0 && (is_eos || cur.part_len[last] > 0)) || cur.part_len[last] > 0) {
             // is_eos=False with an empty next_word is a cache hit on (text, False) as well
             B2cTextNew tn;
-            b2c_text_extend(P, sc->hot, W.text, W.text_cap, cur.text_node[last], cur.part_hash[last], cur.part_len[last], is_eos, &tn, nullptr);
+            b2c_text_extend(M, sc->hot, W.text, W.text_cap, cur.text_node[last], cur.part_hash[last], cur.part_len[last], is_eos, &tn, nullptr);
             lm_hw = tn.lm_hw;
         } else {
             lm_hw = cur.lm_hw[last];
         }
-        const u64 key = keep ? b2c_f64_key(b2c_combine_score(P.lm.order > 0, s, lm_hw, cur.pscore[last], cur.part_len[last]))
-                             : b2c_f64_key(b2c_combine_score(P.lm.order > 0, s, lm_hw, 0.0, 0));
+        const u64 key = keep ? b2c_f64_key(b2c_combine_score(M.lm.order > 0, s, lm_hw, cur.pscore[last], cur.part_len[last]))
+                             : b2c_f64_key(b2c_combine_score(M.lm.order > 0, s, lm_hw, 0.0, 0));
         C.ckey[b] = key;
         b2c_atomic_max_u64(&sc->max_key, key);
     }
@@ -1295,17 +1303,17 @@ B2C_HDN void b2c_finalize(B2cParams P, B2cWork W, B2cOut O, int fin_mode) {
         B2cLmState st;
         st.length = 0;
         for (int w = 0; w < B2C_MAX_HIST; ++w) { st.words[w] = 0; st.backoff[w] = 0.0f; }
-        if (P.lm.order > 0) {
+        if (M.lm.order > 0) {
             if (keep || (!is_eos && cur.part_len[last] == 0)) {
                 st = W.text[cur.text_node[last]].st;
-                if (P.n_lm > 1 && O.states_x) {
-                    const B2cLmState* x = b2c_text_states_x(W.text, W.text_cap, P.n_lm, cur.text_node[last]);
-                    for (int j = 1; j < P.n_lm; ++j) O.states_x[static_cast<u64>(r) * (P.n_lm - 1) + (j - 1)] = x[j - 1];
+                if (M.n_lm > 1 && O.states_x) {
+                    const B2cLmState* x = b2c_text_states_x(W.text, W.text_cap, M.n_lm, cur.text_node[last]);
+                    for (int j = 1; j < M.n_lm; ++j) O.states_x[static_cast<u64>(r) * P.lm_x + (j - 1)] = x[j - 1];
                 }
             } else {
                 B2cTextNew tn;
-                b2c_text_extend(P, sc->hot, W.text, W.text_cap, cur.text_node[last], cur.part_hash[last], cur.part_len[last], is_eos, &tn,
-                                (P.n_lm > 1 && O.states_x) ? O.states_x + static_cast<u64>(r) * (P.n_lm - 1) : nullptr);
+                b2c_text_extend(M, sc->hot, W.text, W.text_cap, cur.text_node[last], cur.part_hash[last], cur.part_len[last], is_eos, &tn,
+                                (M.n_lm > 1 && O.states_x) ? O.states_x + static_cast<u64>(r) * P.lm_x : nullptr);
                 st = tn.st;
             }
         }

@@ -328,7 +328,7 @@ B2C_HD void b2c_fast_commit(const B2cParams& P, B2cFastSmem<WC, CAP, LT>& S, con
     if (word_len > 0) {
         if (flags & B2C_FL_PSCORE) {
             B2cTextCommit tc;
-            b2c_commit_text(P, S.sc.hot, text_arena, text_cap, &S.sc.text_used, &S.sc.status, tnode, cur.part_hash[bl], word_len, &tc);
+            b2c_commit_text(b2c_lm_of(P, &S.sc), S.sc.hot, text_arena, text_cap, &S.sc.text_used, &S.sc.status, tnode, cur.part_hash[bl], word_len, &tc);
             tnode = tc.node;
             lm_hw = tc.lm_hw;
             hh = tc.hist_hash;
@@ -343,7 +343,7 @@ B2C_HD void b2c_fast_commit(const B2cParams& P, B2cFastSmem<WC, CAP, LT>& S, con
     nx.hist_hash[j] = hh;
     double ps = 0.0;
     if (type == 0) ps = cur.pscore[bl];
-    else if (part_len > 0) ps = b2c_partial_score_of(P, S.sc.hot, (flags & B2C_FL_PSCORE) != 0, part_hash, part_len);
+    else if (part_len > 0) ps = b2c_partial_score_of(b2c_lm_of(P, &S.sc), S.sc.hot, (flags & B2C_FL_PSCORE) != 0, part_hash, part_len);
     nx.pscore[j] = ps;
 }
 
@@ -625,12 +625,12 @@ B2C_HD void b2c_fast_step(const B2cParams& P, B2cFastSmem<WC, CAP, LT>& S, B2cCh
             // without LM and hotwords the text-level score is the constant weight * 0 of the empty hotword set: no text node is read
             if ((flags & B2C_FL_PSCORE) && (type == 1 || type == 2) && cur.part_len[bl] > 0) {
                 B2cTextNew tn;
-                b2c_text_extend(P, S.sc.hot, text_arena, text_cap, cur.text_node[bl], cur.part_hash[bl], cur.part_len[bl], 0, &tn, nullptr);
+                b2c_text_extend(b2c_lm_of(P, &S.sc), S.sc.hot, text_arena, text_cap, cur.text_node[bl], cur.part_hash[bl], cur.part_len[bl], 0, &tn, nullptr);
                 lm_hw = tn.lm_hw;
             }
             double ps = 0.0;
             if (type == 0) ps = cur.pscore[bl];
-            else if (part_len > 0) ps = b2c_partial_score_of(P, S.sc.hot, (flags & B2C_FL_PSCORE) != 0, cph & B2C_PH_MASK, part_len);
+            else if (part_len > 0) ps = b2c_partial_score_of(b2c_lm_of(P, &S.sc), S.sc.hot, (flags & B2C_FL_PSCORE) != 0, cph & B2C_PH_MASK, part_len);
             const double sco = b2c_combine_score((flags & B2C_FL_LM) != 0, s, lm_hw, ps, part_len);
             const u64 key = b2c_f64_key(sco);
             S.ckey[i] = key;
@@ -695,8 +695,11 @@ B2C_HD void b2c_fast_step(const B2cParams& P, B2cFastSmem<WC, CAP, LT>& S, B2cCh
                 const u32 meta = S.cmeta[last];
                 u64 hh = cur.hist_hash[bl];
                 if ((type == 1 || type == 2) && cur.part_len[bl] > 0)       // a one-word history does not depend on the parent
-                    hh = P.hist_n == 1 ? b2c_hist_fold(B2C_HIST_SEED, cur.part_hash[bl])
-                                       : b2c_hist_extend(text_arena + cur.text_node[bl], P.hist_n, cur.part_hash[bl]);
+                {
+                    const int hist_n = b2c_lm_of(P, &S.sc).hist_n;
+                    hh = hist_n == 1 ? b2c_hist_fold(B2C_HIST_SEED, cur.part_hash[bl])
+                                     : b2c_hist_extend(text_arena + cur.text_node[bl], hist_n, cur.part_hash[bl]);
+                }
                 const u64 hk = b2c_fast_key(hh, cph & B2C_PH_MASK, meta & 0xFFFFu, meta >> 16);
                 S.phk[rank] = hk;
                 b2c_fence_block();
@@ -904,7 +907,7 @@ B2C_HD bool b2c_fast_scored_step(const B2cParams& P, B2cFastSmem<WC, CAP, LT>& S
     B2C_FOR(b, n) {
         const u64 nph = b2c_hash_append(cur.part_hash[b], ti.raw_hash, ti.raw_pow);
         const u32 nplen = static_cast<u32>(cur.part_len[b]) + ti.raw_nchars;
-        const double ps = b2c_partial_score_of(P, S.sc.hot, true, nph, nplen & 0xFFFFu);
+        const double ps = b2c_partial_score_of(b2c_lm_of(P, &S.sc), S.sc.hot, true, nph, nplen & 0xFFFFu);
         union { double d; u64 u; } c;
         c.d = ps;
         S.ckey[b] = c.u;

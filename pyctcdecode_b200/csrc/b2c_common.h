@@ -164,13 +164,24 @@ struct B2cHotSet {
 
 // MultiLanguageModel (reference language_model.py:455-502): the mean of up to B2C_MAX_LMS n-gram models, each
 // with its own tables, vocabulary, unigram set and alpha / beta / unk offset / boundary flag.  Model 0 lives
-// in B2cParams::lm and the scalar parameters; models 1.. in lmx[].
+// in B2cLmSet::lm and the set's scalar parameters; models 1.. in lmx[].
 #define B2C_MAX_LMS 4
 struct B2cLmExtra {
     B2cLmView lm;
     double alpha, beta, unk_offset;
     int score_boundary;
     int pad;
+};
+// The language model(s) of one utterance: a LanguageModel, a MultiLanguageModel or none (n_lm == 0, lm.order == 0).
+// One descriptor per distinct set of a call, in device memory; an utterance finds its own through B2cParams::utt_lm.
+struct B2cLmSet {
+    B2cLmView lm;              // model 0
+    double alpha, beta, unk_offset, log_base_change;
+    int score_boundary;
+    int hist_n;                // max(1, largest order - 1)   (reference decoder.py:244)
+    int n_lm;                  // 0: none, 1: one model, > 1: MultiLanguageModel (general kernel only)
+    int pad;
+    const B2cLmExtra* lmx;     // [n_lm - 1] models 1..
 };
 
 // ---------------------------------------------------------------------------------------
@@ -182,21 +193,20 @@ struct B2cParams {
     int has_dup_labels;        // two token ids share a label string (their candidates can merge across tokens)
     int beam_width;
     int prune_history;
-    int hist_n;                // max(1, lm order - 1)   (reference decoder.py:244)
+    int lm_x;                  // largest n_lm - 1 of the call's sets: per-beam / per-utterance stride of the states of
+                               // models 1.. (out_states_x), and lm_x + 1 start states per utterance
     int out_beams;             // beams returned per utterance (1 for decode_batch)
     int narrow_chain;          // text-only calls: 8-byte backtrack nodes (no word frames), b2c_chain_store / _load
     double prune_logp;
     double token_min_logp;
-    double alpha, beta, unk_offset, log_base_change;
-    int score_boundary;
     double bucket_scale;       // score buckets per nat for the O(m) ranking (host computed)
     const B2cHotSet* hot_utt;  // [n_utts] hotword set of each utterance, copied into B2cScalars::hot by b2c_utt_begin
     const B2cTok* toks;
-    B2cLmView lm;
-    int n_lm;                  // 0: none, 1: one model, > 1: MultiLanguageModel (general kernel only)
+    const B2cLmSet* lm_sets;   // the call's language-model sets (device memory; the parameter block stays small: it is
+                               // copied into every out-of-line call of the hot kernels)
+    const u32* utt_lm;         // [n_utts] set of each utterance, copied into B2cScalars::lm_set by b2c_utt_begin
     int kflags;                // extra B2C_FL_* mode bits set by the host (B2C_FL_NO_SINGLE: B200CTC_NO_SINGLE_STEP)
-    const B2cLmExtra* lmx;     // [n_lm - 1] models 1.. (device memory; the parameter block stays small: it is copied
-                               // into every out-of-line call of the hot kernels)
+    int pad_params;
 };
 
 // ---------------------------------------------------------------------------------------

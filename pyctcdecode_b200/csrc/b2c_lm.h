@@ -112,9 +112,10 @@ B2C_HD double b2c_lm_score_word_v(const B2cLmView& lm, double alpha, double beta
     }
     return alpha * s * log_base_change + beta;
 }
-B2C_HD double b2c_lm_score_word(const B2cParams& P, const B2cLmState& prev, u64 word_hash, u32 word_len,
+// model 0 of a set
+B2C_HD double b2c_lm_score_word(const B2cLmSet& M, const B2cLmState& prev, u64 word_hash, u32 word_len,
                                 bool is_last, B2cLmState& end_state) {
-    return b2c_lm_score_word_v(P.lm, P.alpha, P.beta, P.unk_offset, P.score_boundary, P.log_base_change, prev, word_hash,
+    return b2c_lm_score_word_v(M.lm, M.alpha, M.beta, M.unk_offset, M.score_boundary, M.log_base_change, prev, word_hash,
                                word_len, is_last, end_state);
 }
 // LanguageModel.score_partial_token of one model (language_model.py:326-336)
@@ -128,17 +129,17 @@ B2C_HD double b2c_lm_partial_v(const B2cLmView& lm, double unk_offset, u64 part_
 
 // score of an unfinished word.  LM mode (reference decoder.py:397-409): hotword prefix score
 // if the partial is a prefix of a hotword, else the LM's OOV-prefix penalty.  No-LM mode
-// (decoder.py:363-367): hotword prefix score or 0.  H: the utterance's hotword set.
-B2C_HD double b2c_partial_score(const B2cParams& P, const B2cHotSet& H, u64 part_hash, u32 part_len) {
+// (decoder.py:363-367): hotword prefix score or 0.  M, H: the utterance's language-model set (model 0) and hotword set.
+B2C_HD double b2c_partial_score(const B2cLmSet& M, const B2cHotSet& H, u64 part_hash, u32 part_len) {
     if (H.min_len > 0) {
         if (part_len == 0) return H.weight * 0 / H.min_len;
         const B2cHot* h = b2c_hot_find(H, part_hash);
         if (h) return H.weight * static_cast<double>(part_len) / static_cast<double>(h->min_len);
     }
-    if (P.lm.order == 0) return 0.0;
+    if (M.lm.order == 0) return 0.0;
     double is_oov = 1.0;
-    if (P.lm.have_unigrams) is_oov = b2c_prefix_contains(P.lm, part_hash) ? 0.0 : 1.0;
-    double unk = P.unk_offset * is_oov;
+    if (M.lm.have_unigrams) is_oov = b2c_prefix_contains(M.lm, part_hash) ? 0.0 : 1.0;
+    double unk = M.unk_offset * is_oov;
     if (part_len > B2C_AVG_TOKEN_LEN) unk = unk * static_cast<double>(part_len) / B2C_AVG_TOKEN_LEN;
     return unk;
 }

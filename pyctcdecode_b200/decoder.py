@@ -141,6 +141,32 @@ def _utt_hot_sets(n: int, hotwords: Optional[Iterable[str]], hotwords_list: Opti
     return out
 
 
+def _models_of(lm: Optional[AbstractLanguageModel]) -> List[LanguageModel]:
+    """[] without a language model, [lm] for a LanguageModel, the member models of a MultiLanguageModel."""
+    if lm is None:
+        return []
+    models = list(lm.language_models) if isinstance(lm, MultiLanguageModel) else [lm]
+    if len(models) > 4:
+        raise ValueError("pyctcdecode_b200 supports at most 4 models in a MultiLanguageModel")
+    for m in models:
+        if not isinstance(m, LanguageModel):
+            raise TypeError("language_model must be a pyctcdecode_b200 LanguageModel (or a MultiLanguageModel of them)")
+    return models
+
+
+def _utt_lm_sets(n: int, language_model_list: Optional[Sequence[Optional[AbstractLanguageModel]]]
+                 ) -> Optional[List[List[LanguageModel]]]:
+    """The models of each of the n utterances of a call with per-utterance language models, None without them."""
+    if language_model_list is None:
+        return None
+    if isinstance(language_model_list, AbstractLanguageModel):
+        raise ValueError("language_model_list holds one language model (or None) per utterance, not a single model")
+    entries = list(language_model_list)
+    if len(entries) != n:
+        raise ValueError("language_model_list has %d entries for %d utterances" % (len(entries), n))
+    return [_models_of(lm) for lm in entries]
+
+
 def _as_matrix(logits: Any) -> Tuple[Any, int, int, int, bool]:
     """-> (owner, address, T, dtype_code, is_device).  float32/float64 are passed through, integer inputs are
     computed in float64 like numpy would, float16 / bfloat16 travel as they are (dtype codes 2 / 3) and are widened
@@ -257,16 +283,7 @@ class BeamSearchDecoderCTC:
 
     def _lm_list(self) -> List[LanguageModel]:
         """[] without a language model, [lm] for a LanguageModel, the member models of a MultiLanguageModel."""
-        lm = self._language_model
-        if lm is None:
-            return []
-        models = list(lm.language_models) if isinstance(lm, MultiLanguageModel) else [lm]
-        if len(models) > 4:
-            raise ValueError("pyctcdecode_b200 supports at most 4 models in a MultiLanguageModel")
-        for m in models:
-            if not isinstance(m, LanguageModel):
-                raise TypeError("language_model must be a pyctcdecode_b200 LanguageModel (or a MultiLanguageModel of them)")
-        return models
+        return _models_of(self._language_model)
 
     def _check_logits_dimension(self, logits: Any) -> None:
         """reference decoder.py:330-344"""
@@ -310,7 +327,8 @@ class BeamSearchDecoderCTC:
              device: Optional[int] = None, texts_only: bool = False, lengths: Optional[Sequence[int]] = None,
              stream: Optional[Sequence[Tuple[Sequence[Beam], int]]] = None, finalize_mode: int = _lib.FIN_EOS,
              hotwords_list: Optional[Sequence[Optional[Iterable[str]]]] = None,
-             hotword_weight_list: Optional[Sequence[float]] = None) -> Any:
+             hotword_weight_list: Optional[Sequence[float]] = None,
+             language_model_list: Optional[Sequence[Optional[AbstractLanguageModel]]] = None) -> Any:
         packed = self._as_packed_batch(logits_list)
         if lengths is not None and packed is None:
             raise ValueError("lengths= needs one padded [B, T, V] array or tensor")
@@ -318,6 +336,7 @@ class BeamSearchDecoderCTC:
             # one [B, T, V] array / tensor: no per-utterance conversion, pointers by arithmetic
             owner, base, n, t_each, dtype_code, is_device = packed
             utt_hot = _utt_hot_sets(n, hotwords, hotwords_list, hotword_weight_list)
+            utt_lms = _utt_lm_sets(n, language_model_list)
             if n == 0:
                 return []
             step = t_each * len(self._idx2vocab) * {0: 4, 1: 8, 2: 2, 3: 2}[dtype_code]
@@ -333,6 +352,7 @@ class BeamSearchDecoderCTC:
                 self._check_logits_dimension(logits)
             n = len(logits_list)
             utt_hot = _utt_hot_sets(n, hotwords, hotwords_list, hotword_weight_list)
+            utt_lms = _utt_lm_sets(n, language_model_list)
             if n == 0:
                 return []
             mats = [_as_matrix(x) for x in logits_list]
@@ -360,14 +380,15 @@ class BeamSearchDecoderCTC:
         with self._run_lock:
             return self._run_locked(mats, n, dtype_code, is_device, device, torch_stream, beam_width, beam_prune_logp,
                                     token_min_logp, prune_history, hotwords, hotword_weight, max_out_beams, lm_start_states,
-                                    with_state, texts_only, stream, finalize_mode, utt_hot)
+                                    with_state, texts_only, stream, finalize_mode, utt_hot, utt_lms)
 
     def _run_locked(self, mats: List[Tuple[Any, int, int, int, bool]], n: int, dtype_code: int, is_device: bool,
                     device: Optional[int], torch_stream: Optional[int], beam_width: int, beam_prune_logp: float,
                     token_min_logp: float, prune_history: bool, hotwords: Optional[Iterable[str]], hotword_weight: float,
                     max_out_beams: int, lm_start_states: Optional[Sequence[Optional[AbstractLMState]]], with_state: bool,
                     texts_only: bool, stream: Optional[Sequence[Tuple[Sequence[Beam], int]]], finalize_mode: int,
-                    utt_hot: Optional[List[Tuple[List[str], float]]] = None) -> Any:
+                    utt_hot: Optional[List[Tuple[List[str], float]]] = None,
+                    utt_lms: Optional[List[List[LanguageModel]]] = None) -> Any:
         handle = self._handle(device)
         lm = self._language_model
         L = _lib.lib()
@@ -406,6 +427,28 @@ class BeamSearchDecoderCTC:
             opts.hot_sets = C.cast(sets, C.POINTER(_lib.HotwordSet))
             opts.n_hot_sets = len(set_of)
             opts.utt_hot_set = C.cast(idx_arr, C.POINTER(C.c_int32))
+        if utt_lms is not None:
+            # parameters are read now (reset_params applies to the next call); utterances whose models are the same
+            # n-gram tables with bit-identical parameters share one set
+            lm_of: Dict[Tuple[Tuple[int, bytes], ...], int] = {}
+            index = []
+            for ms in utt_lms:
+                key = tuple((m.ngram_model._h(), struct.pack("<dddi", float(m.alpha), float(m.beta), float(m.unk_score_offset),
+                                                             int(bool(m.score_boundary)))) for m in ms)
+                index.append(lm_of.setdefault(key, len(lm_of)))
+            lm_sets = (_lib.LmSet * len(lm_of))()
+            for key, k in lm_of.items():
+                lm_sets[k].n_models = len(key)
+                for j, (h, pbits) in enumerate(key):
+                    alpha, beta, unk, boundary = struct.unpack("<dddi", pbits)
+                    lm_sets[k].models[j] = h
+                    lm_sets[k].alpha[j], lm_sets[k].beta[j], lm_sets[k].unk_score_offset[j] = alpha, beta, unk
+                    lm_sets[k].lm_score_boundary[j] = boundary
+            lm_idx = (C.c_int32 * n)(*index)
+            keep_alive += [lm_sets, lm_idx]
+            opts.lm_sets = C.cast(lm_sets, C.POINTER(_lib.LmSet))
+            opts.n_lm_sets = len(lm_of)
+            opts.utt_lm_set = C.cast(lm_idx, C.POINTER(C.c_int32))
         opts.max_out_beams = int(max_out_beams)
         states_arr = None
         n_lm = len(models)
@@ -512,17 +555,25 @@ class BeamSearchDecoderCTC:
                            hotword_weight: float = DEFAULT_HOTWORD_WEIGHT,
                            lengths: Optional[Sequence[int]] = None,
                            hotwords_list: Optional[Sequence[Optional[Iterable[str]]]] = None,
-                           hotword_weight_list: Optional[Sequence[float]] = None) -> List[List[OutputBeam]]:
+                           hotword_weight_list: Optional[Sequence[float]] = None,
+                           language_model_list: Optional[Sequence[Optional[AbstractLanguageModel]]] = None
+                           ) -> List[List[OutputBeam]]:
         """`lengths` (extension, SURVEY 8f-4): valid frames per utterance when `logits_list` is ONE padded
         [B, T, V] array or (CUDA) tensor -- the padding rows are never read.
 
         `hotwords_list` / `hotword_weight_list` (extension): one hotword list (or None) and one weight per utterance.
         Utterance i then gets what ``decode_beams(logits_list[i], hotwords=hotwords_list[i],
-        hotword_weight=hotword_weight_list[i])`` returns, in one batched call."""
+        hotword_weight=hotword_weight_list[i])`` returns, in one batched call.
+
+        `language_model_list` (extension): one LanguageModel, MultiLanguageModel or None per utterance instead of
+        this decoder's own model.  Utterance i then gets what ``BeamSearchDecoderCTC(alphabet,
+        language_model_list[i]).decode_beams(logits_list[i], ...)`` returns, in one batched call; the models'
+        parameters are read at call time."""
         # the reference strips the LM state for multiprocessing (decoder.py:797-799); keep that
         return self._run(logits_list, beam_width, beam_prune_logp, token_min_logp, prune_history, hotwords,
                          hotword_weight, max_out_beams=beam_width, with_state=False, lengths=lengths,
-                         hotwords_list=hotwords_list, hotword_weight_list=hotword_weight_list)
+                         hotwords_list=hotwords_list, hotword_weight_list=hotword_weight_list,
+                         language_model_list=language_model_list)
 
     def decode(self, logits: Any, beam_width: int = DEFAULT_BEAM_WIDTH, beam_prune_logp: float = DEFAULT_PRUNE_LOGP,
                token_min_logp: float = DEFAULT_MIN_TOKEN_LOGP, hotwords: Optional[Iterable[str]] = None,
@@ -535,11 +586,14 @@ class BeamSearchDecoderCTC:
                      beam_prune_logp: float = DEFAULT_PRUNE_LOGP, token_min_logp: float = DEFAULT_MIN_TOKEN_LOGP,
                      hotwords: Optional[Iterable[str]] = None, hotword_weight: float = DEFAULT_HOTWORD_WEIGHT,
                      lengths: Optional[Sequence[int]] = None, hotwords_list: Optional[Sequence[Optional[Iterable[str]]]] = None,
-                     hotword_weight_list: Optional[Sequence[float]] = None) -> List[str]:
-        """`hotwords_list` / `hotword_weight_list` (extension): per-utterance hotwords, as in decode_beams_batch."""
+                     hotword_weight_list: Optional[Sequence[float]] = None,
+                     language_model_list: Optional[Sequence[Optional[AbstractLanguageModel]]] = None) -> List[str]:
+        """`hotwords_list` / `hotword_weight_list` / `language_model_list` (extension): per-utterance hotwords and
+        language models, as in decode_beams_batch."""
         return self._run(logits_list, beam_width, beam_prune_logp, token_min_logp, True, hotwords, hotword_weight,
                          max_out_beams=1, with_state=False, texts_only=True, lengths=lengths,
-                         hotwords_list=hotwords_list, hotword_weight_list=hotword_weight_list)
+                         hotwords_list=hotwords_list, hotword_weight_list=hotword_weight_list,
+                         language_model_list=language_model_list)
 
     # ---- streaming (reference decoder.py:669-728) ------------------------------------------------
     def get_starting_state(self) -> Tuple[List[Beam], LMScoreCache, Dict[str, float]]:

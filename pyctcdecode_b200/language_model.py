@@ -13,6 +13,7 @@ import json
 import logging
 import os
 import shutil
+import threading
 from typing import Any, Collection, Dict, Iterable, List, Optional, Sequence, Set, Tuple
 
 from . import _lib
@@ -115,8 +116,14 @@ class NgramModel:
         self._unigrams = None if unigrams is None else list(unigrams)
         self._handle = _handle
 
+    _build_lock = threading.Lock()     # decoders on several threads may ask for the same model's tables at once
+
     def _h(self) -> int:
-        if self._handle is None:
+        if self._handle is not None:
+            return self._handle
+        with NgramModel._build_lock:
+            if self._handle is not None:
+                return self._handle
             out = C.c_void_p()
             if self._unigrams is None:
                 rc = _lib.lib().b2c_lm_build_from_file(self.path, None, -1, C.byref(out))

@@ -16,7 +16,7 @@ import numpy as np
 from . import _lib
 from .alphabet import Alphabet, verify_alphabet_coverage
 from .constants import DEFAULT_ALPHA, DEFAULT_BETA, DEFAULT_SCORE_LM_BOUNDARY, DEFAULT_UNK_LOGP_OFFSET
-from .decoder import BeamSearchDecoderCTC
+from .decoder import BeamSearchDecoderCTC, _utt_lm_sets
 from .language_model import LanguageModel, NgramModel, load_unigram_set_from_arpa
 
 
@@ -124,12 +124,14 @@ def build_ctcdecoder_broadcast(labels: List[str], kenlm_model_path: Optional[str
 def decode_batch_sharded(decoder: BeamSearchDecoderCTC, logits_list: Sequence[Any], group: Any = None, **kwargs: Any) -> List[str]:
     """Every rank passes the SAME list; each decodes its shard on its own GPU; all ranks return the
     full list of transcripts (one all_gather_object of strings -- not on the data path).  Per-utterance
-    ``hotwords_list`` / ``hotword_weight_list`` are sharded together with the utterances."""
+    ``hotwords_list`` / ``hotword_weight_list`` / ``language_model_list`` are sharded together with the utterances."""
     import torch.distributed as dist
 
     world, rank = dist.get_world_size(group), dist.get_rank(group)
     shards = shard_utterances([x.shape[0] for x in logits_list], world)
-    for key in ("hotwords_list", "hotword_weight_list"):
+    if kwargs.get("language_model_list") is not None:
+        _utt_lm_sets(len(logits_list), kwargs["language_model_list"])   # the decoder's checks, before the list is split
+    for key in ("hotwords_list", "hotword_weight_list", "language_model_list"):
         if kwargs.get(key) is not None:
             per_utt = list(kwargs[key])
             if len(per_utt) != len(logits_list):
