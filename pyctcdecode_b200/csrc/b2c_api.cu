@@ -171,8 +171,8 @@ struct B2cBeamArgs {
     int gate_n;
     int gate_bounds[5];
     u64* phase_clk;            // [16] profiling builds only (-DB2C_PHASE_CLOCKS)
-    u32* m_stats;              // [12] frames over 128..4096 candidates, total frames (adaptive sizing), in-place frames, sorted (no-merge)
-                               // frames, utterances too wide for a one-warp CTA, utterances, single-token-step frames
+    u32* m_stats;              // [10] frames over 128..4096 candidates, total frames (adaptive sizing), in-place frames, sorted (no-merge)
+                               // frames, single-token-step frames
 };
 
 // kFast: every frame of every utterance handed to this launch fits the shared-memory candidate
@@ -293,39 +293,23 @@ B2C_HD void b2c_beam_block(const B2cBeamArgs& A, int slot, u8* smem) {
 // Each variant exists with the label table resident in shared memory (alphabets of up to B2C_FAST_LT labels: runs of
 // in-place frames enabled) and with per-frame label staging (larger alphabets).
 #define B2C_FAST_LT 64
-typedef B2cFastSmem<128, 1024, B2C_FAST_LT> B2cFastSmemA;      // 2 CTAs per SM
-typedef B2cFastSmem<128, 512, B2C_FAST_LT> B2cFastSmemB;       // 3 CTAs per SM
-typedef B2cFastSmem<128, 256, B2C_FAST_LT> B2cFastSmemC;       // 4 CTAs per SM
-// variant 3 is the LEAN one: a one-warp CTA with 32 beam slots and 128 candidates for workloads where few beams stay
-// alive (language model): 8 CTAs per SM; an utterance that needs more is handed back and decoded by a full variant
-typedef B2cFastSmem<32, 128, B2C_FAST_LT> B2cFastSmemL;
-typedef B2cFastSmem<32, 128, 0> B2cFastSmemL0;
-static const u32 kV5Cap[4] = {1024, 512, 256, 128};
-static const int kV5Occ[4] = {2, 3, 4, 8};
-static const int kV5Threads[4] = {128, 128, 128, 32};
+typedef B2cFastSmem<1024, B2C_FAST_LT> B2cFastSmemA;      // 2 CTAs per SM
+typedef B2cFastSmem<512, B2C_FAST_LT> B2cFastSmemB;       // 3 CTAs per SM
+typedef B2cFastSmem<256, B2C_FAST_LT> B2cFastSmemC;       // 4 CTAs per SM
+static const u32 kV5Cap[3] = {1024, 512, 256};
+static const int kV5Occ[3] = {2, 3, 4};
 // [variant][0: staged labels, 1: resident table]
-static const size_t kV5Smem[4][2] = {{sizeof(B2cFastSmem<128, 1024, 0>), sizeof(B2cFastSmemA)},
-                                     {sizeof(B2cFastSmem<128, 512, 0>), sizeof(B2cFastSmemB)},
-                                     {sizeof(B2cFastSmem<128, 256, 0>), sizeof(B2cFastSmemC)},
-                                     {sizeof(B2cFastSmemL0), sizeof(B2cFastSmemL)}};
-static_assert(8 * (sizeof(B2cFastSmemL) + 1024) <= 228 * 1024, "lean variant: 8 CTAs per SM");
+static const size_t kV5Smem[3][2] = {{sizeof(B2cFastSmem<1024, 0>), sizeof(B2cFastSmemA)},
+                                     {sizeof(B2cFastSmem<512, 0>), sizeof(B2cFastSmemB)},
+                                     {sizeof(B2cFastSmem<256, 0>), sizeof(B2cFastSmemC)}};
 // bytes a CTA parks between two chunked launches: everything in front of the per-frame candidate scratch
-typedef B2cFastSmem<128, 1024, 0> B2cFastSmemA0;
-typedef B2cFastSmem<128, 512, 0> B2cFastSmemB0;
-typedef B2cFastSmem<128, 256, 0> B2cFastSmemC0;
-static const size_t kV5Save[4][2] = {{offsetof(B2cFastSmemA0, ckey), offsetof(B2cFastSmemA, ckey)},
+typedef B2cFastSmem<1024, 0> B2cFastSmemA0;
+typedef B2cFastSmem<512, 0> B2cFastSmemB0;
+typedef B2cFastSmem<256, 0> B2cFastSmemC0;
+static const size_t kV5Save[3][2] = {{offsetof(B2cFastSmemA0, ckey), offsetof(B2cFastSmemA, ckey)},
                                      {offsetof(B2cFastSmemB0, ckey), offsetof(B2cFastSmemB, ckey)},
-                                     {offsetof(B2cFastSmemC0, ckey), offsetof(B2cFastSmemC, ckey)},
-                                     {offsetof(B2cFastSmemL0, ckey), offsetof(B2cFastSmemL, ckey)}};
+                                     {offsetof(B2cFastSmemC0, ckey), offsetof(B2cFastSmemC, ckey)}};
 #define B2C_PIPE_CHUNKS 4
-// Features that are ON by default only once a GPU run has validated them (the environment overrides either way:
-// B200CTC_PIPELINE=0/1, B200CTC_LEAN=0/1; read at every call so that tests can switch them).
-#ifndef B2C_DEFAULT_PIPELINE
-#define B2C_DEFAULT_PIPELINE 1
-#endif
-#ifndef B2C_DEFAULT_LEAN
-#define B2C_DEFAULT_LEAN 0
-#endif
 static bool env_switch(const char* name, bool dflt) {
     const char* e = std::getenv(name);
     if (!e || !*e) return dflt;
@@ -371,10 +355,10 @@ B2C_HD void b2c_widen_range(const u16* src, float* dst, u64 begin, u64 end, u64 
 __global__ void __launch_bounds__(256) b2c_widen_kernel(const u16* src, float* dst, u64 n, int bf16) {
     b2c_widen_range(src, dst, static_cast<u64>(blockIdx.x) * blockDim.x + threadIdx.x, n, static_cast<u64>(gridDim.x) * blockDim.x, bf16);
 }
-template <int WC, int CAP, int OCC, int LT>
-__global__ void __launch_bounds__(WC, OCC) b2c_beam_fast_kernel(const B2cBeamArgs A) {
+template <int CAP, int OCC, int LT>
+__global__ void __launch_bounds__(B2C_FAST_WC, OCC) b2c_beam_fast_kernel(const B2cBeamArgs A) {
     extern __shared__ __align__(16) u8 b2c_smem[];
-    b2c_beam_block_fast<WC, CAP, LT>(A, static_cast<int>(blockIdx.x), b2c_smem);
+    b2c_beam_block_fast<CAP, LT>(A, static_cast<int>(blockIdx.x), b2c_smem);
 }
 // device-resident utterances that are not adjacent in memory (a padded [B, T, V] batch with lengths, a list
 // of separate tensors): ONE launch packs their valid rows, instead of one cudaMemcpyAsync per utterance
@@ -579,8 +563,6 @@ struct b2c_decoder {
     int hint_beam = 0, hint_lm = 0, hint_hot = 0, hint_prune = 0;
     u32 hint_over[6] = {0, 0, 0, 0, 0, 0};
     u32 hint_frames = 0;
-    u32 hint_wide_utts = 0, hint_utts = 0;   // utterances of the previous call a one-warp CTA could not have held / all
-    bool lean_bad = false;                   // the lean variant handed back too many utterances for this configuration
 };
 
 struct BeamRes {
@@ -739,21 +721,19 @@ struct Geometry {
 };
 // the B200CTC_* switches (INTEGRATION.md §3), read at every call so that tests can change them between calls
 struct Knobs {
-    bool host_prof, no_pipe, no_hinted, force_v5, no_v5, no_lean, force_lean, pipe_all, no_gate, gate_early, no_single;
+    bool host_prof, no_pipe, no_hinted, force_v5, no_v5, pipe_all, no_gate, gate_early, no_single;
     int v5_variant, force_chunks;  // v5_variant -1: chosen from the hint
 };
 static bool env_set(const char* name) { return std::getenv(name) != nullptr; }
 static Knobs read_knobs() {
     Knobs k;
     k.host_prof = env_set("B200CTC_HOST_PROFILE");        // host-side section timing on stderr
-    k.no_pipe = env_set("B200CTC_NO_PIPELINE") || !env_switch("B200CTC_PIPELINE", B2C_DEFAULT_PIPELINE != 0);
+    k.no_pipe = env_set("B200CTC_NO_PIPELINE") || !env_switch("B200CTC_PIPELINE", true);
     k.no_hinted = env_set("B200CTC_NO_HINTED");
     k.force_v5 = env_set("B200CTC_FORCE_V5");             // tests: exercise the out-of-line step
     k.no_v5 = env_set("B200CTC_NO_V5");
     const char* v = std::getenv("B200CTC_V5_VARIANT"), *fc = std::getenv("B200CTC_FORCE_CHUNKS");
     k.v5_variant = v ? std::max(0, std::min(2, std::atoi(v))) : -1;
-    k.no_lean = env_set("B200CTC_NO_LEAN") || !env_switch("B200CTC_LEAN", B2C_DEFAULT_LEAN != 0);
-    k.force_lean = env_set("B200CTC_FORCE_LEAN");
     k.force_chunks = fc ? std::atoi(fc) : 0;              // tests
     k.pipe_all = env_set("B200CTC_PIPELINE_ALL"); k.no_gate = env_set("B200CTC_NO_GATE");
     k.gate_early = env_set("B200CTC_HOSTSIM_GATE_EARLY");  // hostsim tests: the later chunks of a gated launch never arrive
@@ -763,7 +743,7 @@ static Knobs read_knobs() {
 struct Plan {
     std::vector<Launch> launches;
     std::vector<int> ord;         // the work list: utterances of the launches, launch by launch
-    bool use_v5 = false, use_lean = false;
+    bool use_v5 = false;
     int v5_variant = 0;
     std::vector<int> bounds;      // chunk boundaries along T ({0, T_max}: one chunk)
     bool gated = false;           // chunks feed ONE beam launch through device flags
@@ -948,30 +928,27 @@ static int launch_beam(b2c_decoder* d, const B2cBeamArgs& A, const Launch& ln, c
     std::vector<u8> smem(A.L.smem_bytes + 64);
     const bool table = A.P.V <= B2C_FAST_LT;
     for (int s = 0; s < slots; ++s) {
-        if (v5 == 0) table ? b2c_beam_block_fast<128, 1024, B2C_FAST_LT>(A, s, smem.data()) : b2c_beam_block_fast<128, 1024, 0>(A, s, smem.data());
-        else if (v5 == 1) table ? b2c_beam_block_fast<128, 512, B2C_FAST_LT>(A, s, smem.data()) : b2c_beam_block_fast<128, 512, 0>(A, s, smem.data());
-        else if (v5 == 2) table ? b2c_beam_block_fast<128, 256, B2C_FAST_LT>(A, s, smem.data()) : b2c_beam_block_fast<128, 256, 0>(A, s, smem.data());
-        else if (v5 == 3) table ? b2c_beam_block_fast<32, 128, B2C_FAST_LT>(A, s, smem.data()) : b2c_beam_block_fast<32, 128, 0>(A, s, smem.data());
+        if (v5 == 0) table ? b2c_beam_block_fast<1024, B2C_FAST_LT>(A, s, smem.data()) : b2c_beam_block_fast<1024, 0>(A, s, smem.data());
+        else if (v5 == 1) table ? b2c_beam_block_fast<512, B2C_FAST_LT>(A, s, smem.data()) : b2c_beam_block_fast<512, 0>(A, s, smem.data());
+        else if (v5 == 2) table ? b2c_beam_block_fast<256, B2C_FAST_LT>(A, s, smem.data()) : b2c_beam_block_fast<256, 0>(A, s, smem.data());
         else if (fast) b2c_beam_block<true>(A, s, smem.data());
         else b2c_beam_block<false>(A, s, smem.data());
     }
 #else
     const int smem = static_cast<int>(A.L.smem_bytes);
-#define B2C_LAUNCH_V5(WC, CAP, OCC, LT)                                                                                 \
+#define B2C_LAUNCH_V5(CAP, OCC, LT)                                                                                     \
     do {                                                                                                               \
-        CUDA_OK(cudaFuncSetAttribute(b2c_beam_fast_kernel<WC, CAP, OCC, LT>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)); \
-        b2c_beam_fast_kernel<WC, CAP, OCC, LT><<<slots, WC, A.L.smem_bytes, stream>>>(A);                             \
+        CUDA_OK(cudaFuncSetAttribute(b2c_beam_fast_kernel<CAP, OCC, LT>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)); \
+        b2c_beam_fast_kernel<CAP, OCC, LT><<<slots, B2C_FAST_WC, A.L.smem_bytes, stream>>>(A);                        \
     } while (0)
     if (v5 >= 0) {
         const bool table = A.P.V <= B2C_FAST_LT;
-        if (v5 == 0 && table) B2C_LAUNCH_V5(128, 1024, 2, B2C_FAST_LT);
-        else if (v5 == 0) B2C_LAUNCH_V5(128, 1024, 2, 0);
-        else if (v5 == 1 && table) B2C_LAUNCH_V5(128, 512, 3, B2C_FAST_LT);
-        else if (v5 == 1) B2C_LAUNCH_V5(128, 512, 3, 0);
-        else if (v5 == 2 && table) B2C_LAUNCH_V5(128, 256, 4, B2C_FAST_LT);
-        else if (v5 == 2) B2C_LAUNCH_V5(128, 256, 4, 0);
-        else if (table) B2C_LAUNCH_V5(32, 128, 8, B2C_FAST_LT);
-        else B2C_LAUNCH_V5(32, 128, 8, 0);
+        if (v5 == 0 && table) B2C_LAUNCH_V5(1024, 2, B2C_FAST_LT);
+        else if (v5 == 0) B2C_LAUNCH_V5(1024, 2, 0);
+        else if (v5 == 1 && table) B2C_LAUNCH_V5(512, 3, B2C_FAST_LT);
+        else if (v5 == 1) B2C_LAUNCH_V5(512, 3, 0);
+        else if (table) B2C_LAUNCH_V5(256, 4, B2C_FAST_LT);
+        else B2C_LAUNCH_V5(256, 4, 0);
         CUDA_OK(cudaGetLastError());
         return 0;
     }
@@ -1021,20 +998,14 @@ static Launch plan_launch(const Geometry& g, const u32* maxk, const Plan& p, int
         kmax = std::max(kmax, maxk[u]);
     }
     const u64 worst_m = static_cast<u64>(g.W_tab) * std::min<u32>(kmax, static_cast<u32>(g.V));
-    ln.v5 = (p.use_v5 && cls < kNumCaps) ? (p.use_lean ? 3 : p.v5_variant) : -1;
-    if (ln.v5 == 3) {
-        // lean variant: 32 slots, 128 candidates, no out-of-line tier (what does not fit is handed back)
-        ln.threads = 32;
-        ln.L = make_layout(32, g.V, tmax, full, g.smem_budget, 128, 0, 1);
-        ln.L.smem_bytes = static_cast<u32>(kV5Smem[3][g.V <= B2C_FAST_LT ? 1 : 0]);
-        ln.per_sm = kV5Occ[3];
-    } else if (ln.v5 >= 0) {
+    ln.v5 = (p.use_v5 && cls < kNumCaps) ? p.v5_variant : -1;
+    if (ln.v5 >= 0) {
         // beam tables of capacity 128; the HBM tier always exists (frames with more tokens than the rings hold use it too)
         const u32 cap5 = kV5Cap[ln.v5];
-        ln.threads = kV5Threads[ln.v5];
-        // backtrack arena: fixed node ids of the frame steps below 128 * T, the out-of-line step allocates above
-        ln.L = make_layout(128, g.V, tmax, full, g.smem_budget, cap5, std::max<u64>(worst_m, cap5 + 1), B2C_FAST_NW,
-                           128ull * static_cast<u64>(std::max(tmax, 1)));
+        ln.threads = B2C_FAST_WC;
+        // backtrack arena: fixed node ids of the frame steps below B2C_FAST_WC * T, the out-of-line step allocates above
+        ln.L = make_layout(B2C_FAST_WC, g.V, tmax, full, g.smem_budget, cap5, std::max<u64>(worst_m, cap5 + 1), B2C_FAST_NW,
+                           static_cast<u64>(B2C_FAST_WC) * static_cast<u64>(std::max(tmax, 1)));
         ln.L.smem_bytes = static_cast<u32>(kV5Smem[ln.v5][g.V <= B2C_FAST_LT ? 1 : 0]);
         ln.per_sm = kV5Occ[ln.v5];
     } else {
@@ -1161,11 +1132,6 @@ static Plan make_plan(const Geometry& g, const u32* maxk, const u32* sumk, const
         }
     }
     if (k.v5_variant >= 0) p.v5_variant = k.v5_variant;
-    // the lean one-warp variant: more utterances than the chosen variant keeps resident, and the previous call of
-    // this configuration says that (nearly) every utterance fits 32 slots / 128 candidates / 16 tokens per frame
-    p.use_lean = p.use_v5 && g.beam_width <= 128 &&
-                 (k.force_lean || (!k.no_lean && (g.hint_ok && !d.lean_bad && d.hint_utts > 0 && 20ull * d.hint_wide_utts <= d.hint_utts &&
-                                                 n_fast > d.n_sm * kV5Occ[p.v5_variant])));
     std::vector<std::vector<int>> classes(kNumCaps + 1);   // the fast class (one per call), last = general
     for (int q = 0; q < g.n_utts; ++q) {
         const int u = g.order[q];             // keeps longest-first order inside every class
@@ -2076,51 +2042,35 @@ static int read_back(b2c_decoder* d, Call& c) {
     for (int q = 0; q < 6; ++q) d->hint_over[q] = ms[q];
     d->hint_frames = ms[6];
     for (int q = 0; q < 7; ++q) d->tm.cand_hist[q] = ms[q];
-    d->tm.inplace_frames = ms[7]; d->tm.sorted_frames = ms[8]; d->tm.single_frames = ms[11];
-    d->hint_wide_utts = ms[9]; d->hint_utts = ms[10];
+    d->tm.inplace_frames = ms[7]; d->tm.sorted_frames = ms[8]; d->tm.single_frames = ms[9];
     d->tm.oversize_frames = 0;
     for (int q = 0; q < 6; ++q)
         if (static_cast<int>(128u << q) == d->tm.cap_candidates) d->tm.oversize_frames = ms[q];
     return 0;
 }
 
-// retry passes: (1) utterances the lean variant handed back -> a full latency-first variant; (2) utterances whose
-// arenas overflowed -> the general kernel with worst-case arenas
+// retry pass: utterances whose arenas overflowed are decoded again by the general kernel with worst-case arenas
 static int retry_failed(b2c_decoder* d, Call& c) {
     const int n = c.g.n_utts;
     cudaStream_t st = d->stream;
     const int* status = c.out.at(d->h_out_small.as<u8>()).status;
     std::vector<int> failed;
     for (int i = 0; i < n; ++i) if (status[i] != B2C_OK) failed.push_back(i);
-    if (c.plan.use_lean && 10 * failed.size() > static_cast<size_t>(n)) d->lean_bad = true;     // not worth it for this configuration
-    for (int pass = 0; pass < 2 && !failed.empty(); ++pass) {
-        bool only_slots = c.plan.use_lean && pass == 0;
-        for (int i : failed) only_slots = only_slots && status[i] == B2C_ERR_SLOTS;
-        if (pass == 0 && !only_slots) continue;
-        int cls = kNumCaps;
-        if (only_slots) {
-            c.plan.use_lean = false;
-            cls = 0;
-            for (const Launch& l0 : c.plan.launches) if (l0.v5 >= 0) cls = l0.cls;
-        }
-        const Launch ln = plan_launch(c.g, c.maxk, c.plan, d->n_sm, failed, cls, !only_slots, static_cast<size_t>(n));
-        if (ln.L.smem_bytes > d->smem_optin) return fail(B2C_E_ARG, "beam_width too large for the shared-memory selection arrays");
-        if (d->d_ws.ensure(static_cast<u64>(ln.slots) * ln.L.gws_bytes)) return B2C_E_NOMEM;
-        int* h_ord = c.h_ord();
-        for (size_t i = 0; i < failed.size(); ++i) h_ord[n + i] = failed[i];
-        CUDA_OK(cudaMemcpyAsync(c.d_ord() + n, h_ord + n, 4 * failed.size(), cudaMemcpyHostToDevice, st));
-        CUDA_OK(cudaMemsetAsync(c.d_next() + 15, 0, 4, st));
-        c.BA.L = ln.L; c.BA.n_utts = ln.count; c.BA.order = c.d_ord() + n; c.BA.next = c.d_next() + 15; c.BA.gws = d->d_ws.as<u8>();
-        c.BA.chunk_t1 = 0;
-        B2C_TRY(launch_beam(d, c.BA, ln, st, false));
-        B2C_TRY(read_outputs(d, c, true));
-        CUDA_OK(cudaStreamSynchronize(st));
-        std::vector<int> still;
-        for (int i : failed) if (status[i] != B2C_OK) still.push_back(i);
-        failed.swap(still);
-    }
+    if (failed.empty()) return 0;
+    const Launch ln = plan_launch(c.g, c.maxk, c.plan, d->n_sm, failed, kNumCaps, true, static_cast<size_t>(n));
+    if (ln.L.smem_bytes > d->smem_optin) return fail(B2C_E_ARG, "beam_width too large for the shared-memory selection arrays");
+    if (d->d_ws.ensure(static_cast<u64>(ln.slots) * ln.L.gws_bytes)) return B2C_E_NOMEM;
+    int* h_ord = c.h_ord();
+    for (size_t i = 0; i < failed.size(); ++i) h_ord[n + i] = failed[i];
+    CUDA_OK(cudaMemcpyAsync(c.d_ord() + n, h_ord + n, 4 * failed.size(), cudaMemcpyHostToDevice, st));
+    CUDA_OK(cudaMemsetAsync(c.d_next() + 15, 0, 4, st));
+    c.BA.L = ln.L; c.BA.n_utts = ln.count; c.BA.order = c.d_ord() + n; c.BA.next = c.d_next() + 15; c.BA.gws = d->d_ws.as<u8>();
+    c.BA.chunk_t1 = 0;
+    B2C_TRY(launch_beam(d, c.BA, ln, st, false));
+    B2C_TRY(read_outputs(d, c, true));
+    CUDA_OK(cudaStreamSynchronize(st));
     for (int i : failed)
-        return fail(B2C_E_INTERNAL, "beam kernel workspace overflow (status " + std::to_string(status[i]) + ")");
+        if (status[i] != B2C_OK) return fail(B2C_E_INTERNAL, "beam kernel workspace overflow (status " + std::to_string(status[i]) + ")");
     return 0;
 }
 

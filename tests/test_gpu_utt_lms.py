@@ -1,8 +1,7 @@
 """Per-utterance language models on the device (tests/utt_lms.py): every batched result equals, bit for bit, the
 single-utterance call on a decoder built with that utterance's model, and the oracle per group of utterances sharing a
-single-model set; in each latency-first variant, the lean variant and the general kernel, with padded, pipelined,
-chunked and device-resident input, together with per-utterance hotwords, and in mixed batches that keep the special
-steps."""
+single-model set; in each latency-first variant and the general kernel, with padded, pipelined, chunked and
+device-resident input, together with per-utterance hotwords, and in mixed batches that keep the special steps."""
 import threading
 
 import pytest
@@ -49,20 +48,17 @@ def test_gpu_utt_lms_contract(pkg, char_sets, kind, prune_history):
     ul.check_oracle(sets, oracle, xs, names, got, beam_width=24, prune_history=prune_history)
 
 
-@pytest.mark.parametrize("variant", ["0", "1", "2", "lean", "general"])
+@pytest.mark.parametrize("variant", ["0", "1", "2", "general"])
 def test_gpu_utt_lms_kernels(pkg, char_sets, variant, monkeypatch):
     if variant == "general":
         bw = 160                  # above the latency-first kernel's 128 beams
-    elif variant == "lean":
-        monkeypatch.setenv("B200CTC_FORCE_LEAN", "1")
-        bw = 16
     else:
         monkeypatch.setenv("B200CTC_FORCE_V5", "1")
         monkeypatch.setenv("B200CTC_V5_VARIANT", variant)
         bw = 32
     # a MultiLanguageModel set sends the whole call to the general kernel
     names = char_sets.names(16, ul.NAMES if variant == "general" else ["A", "B", "A_params", "A_no_unigrams", "none"])
-    dec = _decoder(pkg, char_sets, own=None if variant == "lean" else "A")
+    dec = _decoder(pkg, char_sets)
     xs = ul.batch(char_sets.wl, n=16)
     ul.check_contract(char_sets, dec, xs, char_sets.models(names), beam_width=bw)
     ul.check_route(dec, variant)

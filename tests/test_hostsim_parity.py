@@ -595,18 +595,6 @@ def test_hostsim_pipelined_host_batches(sim, fam, dtype, monkeypatch):
     assert dec.decode_batch(None, probs, beam_width=24) == want_p
 
 
-def test_hostsim_lean_variant_with_hand_back():
-    """The lean one-warp variant of the latency-first kernel (32 beam slots, 128 candidates) forced for every call
-    (B200CTC_FORCE_LEAN): utterances that need more are handed back with an error status and decoded again by a full
-    variant (host retry pass) -- the parity tests must pass unchanged."""
-    import sys
-    env = dict(os.environ, B200CTC_FORCE_LEAN="1", B200CTC_FORCE_V5="1")
-    here = os.path.abspath(__file__)
-    r = subprocess.run([sys.executable, "-m", "pytest", here, "-x", "-q", "-k", "golden or special or random or ragged or text_only or scored"],
-                       env=env, cwd=os.path.dirname(os.path.dirname(here)), stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
-    assert r.returncode == 0, r.stdout[-3000:]
-
-
 def test_hostsim_gated_launch_gives_up_cleanly(sim, monkeypatch):
     """A gated launch whose later chunks never become ready (here: hostsim launches the beam kernel right after the
     first chunk) must give up with B2C_ERR_GATE -- no hang, no garbage -- and the call is redone as a plain call."""

@@ -48,20 +48,17 @@ def test_hostsim_utt_lms_contract(sim, char_sets, kind, prune_history):
     ul.check_oracle(sets, orc, xs, names, got, beam_width=24, prune_history=prune_history)
 
 
-@pytest.mark.parametrize("variant", ["0", "1", "2", "lean", "general"])
+@pytest.mark.parametrize("variant", ["0", "1", "2", "general"])
 def test_hostsim_utt_lms_kernels(sim, char_sets, variant, monkeypatch):
     if variant == "general":
         bw = 160                  # above the latency-first kernel's 128 beams
-    elif variant == "lean":
-        monkeypatch.setenv("B200CTC_FORCE_LEAN", "1")
-        bw = 16
     else:
         monkeypatch.setenv("B200CTC_FORCE_V5", "1")
         monkeypatch.setenv("B200CTC_V5_VARIANT", variant)
         bw = 32
     # a MultiLanguageModel set sends the whole call to the general kernel
     names = char_sets.names(12, ul.NAMES if variant == "general" else ["A", "B", "A_params", "A_no_unigrams", "none"])
-    dec = _decoder(sim, char_sets, own=None if variant == "lean" else "A")
+    dec = _decoder(sim, char_sets)
     xs = ul.batch(char_sets.wl)
     ul.check_contract(char_sets, dec, xs, char_sets.models(names), beam_width=bw)
     ul.check_route(dec, variant)

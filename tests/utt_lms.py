@@ -134,14 +134,13 @@ def mixed_special_steps(sets, dec, xs, **kw):
 
 
 def check_route(dec, variant):
-    """The last call ran the kernel the test forced: the general kernel, the lean one-warp variant or a latency-first
-    variant."""
+    """The last call ran the kernel the test forced: the general kernel or a latency-first variant."""
     tm = dec.last_timings()
     if variant == "general":
         assert tm["kernel_variant"] == 0
     else:
         assert tm["kernel_variant"] == 2
-        assert (tm["cta_threads"] == 32) == (variant == "lean")
+        assert tm["cta_threads"] == 128
 
 
 def check_pipelined(sets, dec, xs, lms, block, monkeypatch, **kw):
