@@ -155,7 +155,13 @@ typedef struct {
     int n_hotwords;
     double hotword_weight;     /* DEFAULT_HOTWORD_WEIGHT 10       (constants.py:9)  */
     int max_out_beams;         /* 1 for decode()/decode_batch(); beam_width for decode_beams*() */
-    const b2c_lm_state_t* lm_start_states; /* NULL, or one start state per utterance (lm_start_state, decoder.py:612-625) */
+    /* NULL, or the start states (lm_start_state, decoder.py:612-625): n_utts rows of W states, W = the number of models
+     * of the call's largest set (the decoder's own models without utt_lm_set; at least 1).  Utterance i uses the first
+     * n_models entries of its row, one per model of its own set in set order; the rest of the row, and the whole row of
+     * an utterance without a model, is not read.  Every state that is read is checked on the host before anything is
+     * enqueued: B2C_E_ARG for a length above 5 or for a word id among the first `length` that is not below its model's
+     * vocabulary size.  A state of another model whose ids all lie inside the vocabulary cannot be told apart. */
+    const b2c_lm_state_t* lm_start_states;
     /* streaming (partial_decode_beams, decoder.py:669-728): NULL, or one state per utterance = the beams the call
      * starts from (NULL beams / n_beams == 0: EMPTY_START_BEAM) and processed_frames */
     const struct b2c_stream_state* stream_states;
@@ -173,13 +179,20 @@ typedef struct {
     /* per-utterance language models: utterance i is decoded exactly as a call of its own on a decoder created with the
      * models of lm_sets[utt_lm_set[i]] (and their parameters).  utt_lm_set NULL: every utterance uses the decoder's
      * own model(s) and lm_sets is not read.  Models are uploaded to the decoder's device on first use.  B2C_E_ARG: an
-     * index outside [0, n_lm_sets), a set with a NULL model or with n_models outside [0, 4], or utt_lm_set together
-     * with lm_start_states or stream_states.  Results: b2c_result_lm_state(_at) return the states of the utterance's
+     * index outside [0, n_lm_sets), or a set with a NULL model or with n_models outside [0, 4].  Composes with
+     * lm_start_states (layout above; lm_start_width must state W) and with stream_states: a streaming utterance starts
+     * from its row of lm_start_states, which a streaming call with utt_lm_set must give (B2C_E_ARG without it), and
+     * replays the words of its input beams through its own set.  Streaming calls and calls with a set of more
+     * than one model run on the general kernel.  Results: b2c_result_lm_state(_at) return the states of the utterance's
      * own set (0 for an utterance without a model); in b2c_packed_t n_models is the largest set of the call, and a
      * beam of a smaller set has its models' states first, then zeroed states (length 0). */
     const struct b2c_lm_set* lm_sets;
     int n_lm_sets;
     const int32_t* utt_lm_set; /* NULL, or [n_utts] indices into lm_sets */
+    /* W of the lm_start_states layout, stated by the caller when utt_lm_set is given together with lm_start_states: it
+     * must equal the number of models of the call's largest set (at least 1), else B2C_E_ARG (the library cannot see
+     * the extent of the array).  Not read without utt_lm_set. */
+    int lm_start_width;
 } b2c_decode_opts_t;
 void b2c_decode_opts_default(b2c_decode_opts_t* opts);
 

@@ -62,6 +62,7 @@ class DecodeOpts(C.Structure):
         ("lm_sets", C.POINTER(LmSet)),
         ("n_lm_sets", C.c_int),
         ("utt_lm_set", C.POINTER(C.c_int32)),
+        ("lm_start_width", C.c_int),
     ]
 
 

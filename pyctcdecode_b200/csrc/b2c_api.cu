@@ -1548,7 +1548,6 @@ static int make_lm(b2c_decoder* d, Call& c) {
     struct Model { b2c_lm* lm; double alpha, beta, unk; int score_boundary; };
     std::vector<std::vector<Model>> models;
     if (o->utt_lm_set) {
-        if (o->lm_start_states || o->stream_states) return fail(B2C_E_ARG, "opts->utt_lm_set excludes lm_start_states and stream_states");
         if (o->n_lm_sets < 0 || (o->n_lm_sets > 0 && !o->lm_sets)) return fail(B2C_E_ARG, "null lm_sets");
         for (int i = 0; i < n; ++i)
             if (o->utt_lm_set[i] < 0 || o->utt_lm_set[i] >= o->n_lm_sets) return fail(B2C_E_ARG, "utt_lm_set index out of range");
@@ -1573,6 +1572,36 @@ static int make_lm(b2c_decoder* d, Call& c) {
     const int n_sets = static_cast<int>(models.size());
     std::vector<char> used(static_cast<size_t>(n_sets), o->utt_lm_set ? 0 : 1);
     for (int i = 0; o->utt_lm_set && i < n; ++i) used[o->utt_lm_set[i]] = 1;
+    // Every start state the kernels will read, checked against the model of its slot before anything is uploaded (layout:
+    // include/b200ctc.h, lm_start_states).  b2c_lm_base_score reads backoff[0, length) and hashes the word ids: a length
+    // above B2C_MAX_HIST would index past the state, an id outside the vocabulary belongs to another model.
+    size_t width = 1;
+    for (int k = 0; k < n_sets; ++k)
+        if (used[k]) width = std::max(width, models[k].size());
+    if (o->utt_lm_set) {
+        // with per-utterance sets the caller states the row width of its array (the library cannot see its extent), and
+        // a streaming call gives every stream's start state, as the reference reads it from the stream's cache
+        if (o->stream_states && !o->lm_start_states)
+            return fail(B2C_E_ARG, "a streaming call with utt_lm_set needs lm_start_states (one row per stream)");
+        if (o->lm_start_states && o->lm_start_width != static_cast<int>(width))
+            return fail(B2C_E_ARG, "lm_start_width is " + std::to_string(o->lm_start_width) + ": with utt_lm_set it must be " +
+                                       std::to_string(width) + ", the models of the call's largest set");
+    }
+    if (o->lm_start_states) {
+        for (int i = 0; i < n; ++i) {
+            const std::vector<Model>& ms = models[o->utt_lm_set ? o->utt_lm_set[i] : 0];
+            for (size_t j = 0; j < ms.size(); ++j) {
+                const b2c_lm_state_t& s = o->lm_start_states[static_cast<size_t>(i) * width + j];
+                const u32 n_vocab = ms[j].lm->host.header()->n_vocab;
+                bool ok = s.length <= B2C_MAX_HIST;
+                for (u32 w = 0; ok && w < s.length; ++w) ok = s.words[w] < n_vocab;
+                if (!ok)
+                    return fail(B2C_E_ARG, "lm_start_states: the state of utterance " + std::to_string(i) + ", model " + std::to_string(j) +
+                                               " has more than 5 words or a word id outside the model's vocabulary of " +
+                                               std::to_string(n_vocab));
+            }
+        }
+    }
     std::vector<B2cLmSet> sets(static_cast<size_t>(std::max(n_sets, 1)));
     std::vector<B2cLmExtra> extra;
     std::vector<size_t> x_off(static_cast<size_t>(n_sets), 0);

@@ -1633,6 +1633,7 @@ B2C_HD void b2c_beam_block_fast(const B2cBeamArgs& A, int slot_cta, u8* smem) {
         } else {
             B2cWork W;
             b2c_fast_work(S, L, g, 0, false, W);
+            // stride 1 = P.lm_x + 1: this kernel runs only when no set of the call holds more than one model (plan_launch)
             b2c_utt_begin(A.P, W, u, A.start_states ? A.start_states + u : nullptr, 1, B2cStreamIn{nullptr, 0u, nullptr, nullptr});
         }
         B2C_FOR(s, SM::HT + 1) {

@@ -390,7 +390,6 @@ class BeamSearchDecoderCTC:
                     utt_hot: Optional[List[Tuple[List[str], float]]] = None,
                     utt_lms: Optional[List[List[LanguageModel]]] = None) -> Any:
         handle = self._handle(device)
-        lm = self._language_model
         L = _lib.lib()
         if torch_stream is not None:
             # the logits may still be in flight on torch's current stream: the decoder's stream waits for it
@@ -452,21 +451,32 @@ class BeamSearchDecoderCTC:
         opts.max_out_beams = int(max_out_beams)
         states_arr = None
         n_lm = len(models)
-        if lm is not None and lm_start_states is not None and any(s is not None for s in lm_start_states):
-            states_arr = (_lib.LMState * (n * n_lm))()      # n_lm consecutive states per utterance
-            for i, s in enumerate(lm_start_states):
-                st = s if s is not None else lm.get_start_state()
-                if n_lm > 1:
-                    if not isinstance(st, MultiLanguageModelState) or len(st.states) != n_lm:
+        utt_models = utt_lms if utt_lms is not None else [models] * n
+        # with per-utterance sets (streaming only: the offline calls take no start states) every row is given
+        if lm_start_states is not None and (utt_lms is not None or
+                                            any(s is not None and ms for s, ms in zip(lm_start_states, utt_models))):
+            # a row of `width` states per utterance; utterance i fills the first len(utt_models[i]) with its own models'
+            # states (include/b200ctc.h, lm_start_states); an utterance without a model ignores its entry
+            width = max(1, max(len(ms) for ms in utt_models))
+            opts.lm_start_width = width
+            states_arr = (_lib.LMState * (n * width))()
+            for i, (s, ms) in enumerate(zip(lm_start_states, utt_models)):
+                if not ms:
+                    continue
+                k = len(ms)
+                st = s if s is not None else (ms[0].get_start_state() if k == 1 else
+                                              MultiLanguageModelState([m.get_start_state() for m in ms]))
+                if k > 1:
+                    if not isinstance(st, MultiLanguageModelState) or len(st.states) != k:
                         raise AssertionError("Wrong input state type found. Expected MultiLanguageModelState with %d states, "
-                                             "got %s" % (n_lm, type(st)))
+                                             "got %s" % (k, type(st)))
                     parts = list(st.states)
                 else:
                     parts = [st]
                 for j, part in enumerate(parts):
                     if not isinstance(part, B200LMState):
                         raise AssertionError("Wrong input state type found. Expected B200LMState, got %s" % type(part))
-                    states_arr[i * n_lm + j] = part._to_c()
+                    states_arr[i * width + j] = part._to_c()
             opts.lm_start_states = C.cast(states_arr, C.POINTER(_lib.LMState))
         if stream is not None:
             opts.stream_states = C.cast(self._stream_states(handle, stream, keep_alive), C.POINTER(_lib.StreamState))
@@ -596,11 +606,18 @@ class BeamSearchDecoderCTC:
                          language_model_list=language_model_list)
 
     # ---- streaming (reference decoder.py:669-728) ------------------------------------------------
-    def get_starting_state(self) -> Tuple[List[Beam], LMScoreCache, Dict[str, float]]:
+    def get_starting_state(self, language_model: Optional[AbstractLanguageModel] = None
+                           ) -> Tuple[List[Beam], LMScoreCache, Dict[str, float]]:
         """Starting beams and caches, same shape as the reference returns (decoder.py:669-680).  The caches are
         accepted back by partial_decode_beams for signature compatibility; only the start state stored under
-        ("", False) is read -- the kernels recompute LM / hotword scores of the carried beams from their words."""
-        language_model = self._language_model
+        ("", False) is read -- the kernels recompute LM / hotword scores of the carried beams from their words.
+
+        `language_model` (extension): what ``BeamSearchDecoderCTC(alphabet, language_model).get_starting_state()``
+        returns, for a stream that partial_decode_beams_batch decodes with its own model (`language_model_list`)."""
+        if language_model is None:
+            language_model = self._language_model
+        else:
+            _models_of(language_model)      # the errors of language_model_list
         cached_lm_scores: LMScoreCache = {}
         if language_model is not None:
             cached_lm_scores[("", False)] = (0.0, 0.0, language_model.get_start_state())
@@ -850,9 +867,18 @@ class BeamSearchDecoderCTC:
                                    token_min_logp: float = DEFAULT_MIN_TOKEN_LOGP, prune_history: bool = DEFAULT_PRUNE_BEAMS,
                                    hotword_scorer: Optional[HotwordScorer] = None, force_next_word: bool = False,
                                    is_end: bool = False,
-                                   hotword_scorer_list: Optional[Sequence[Optional[HotwordScorer]]] = None) -> List[List[LMBeam]]:
+                                   hotword_scorer_list: Optional[Sequence[Optional[HotwordScorer]]] = None,
+                                   language_model_list: Optional[Sequence[Optional[AbstractLanguageModel]]] = None
+                                   ) -> List[List[LMBeam]]:
         """Extension: many independent streams advance by one chunk each in ONE kernel launch.  `hotword_scorer_list`:
-        one HotwordScorer (or None) per stream instead of one `hotword_scorer` for all."""
+        one HotwordScorer (or None) per stream instead of one `hotword_scorer` for all.
+
+        `language_model_list`: one LanguageModel, MultiLanguageModel or None per stream instead of this decoder's own
+        model.  Stream i then gets what ``BeamSearchDecoderCTC(alphabet, language_model_list[i]).partial_decode_beams``
+        returns for it.  The words its beams carry are replayed through the model of this call, so a stream may change
+        its model between calls.  Its start state is read from its cache under ("", False): a MultiLanguageModelState
+        of k states for a set of k models, a B200LMState for one; get_starting_state(language_model=...) makes it, and
+        a missing entry means that model's default start state."""
         n = len(logits_list)
         if not (len(beams_list) == len(processed_frames_list) == len(cached_lm_scores_list) == n):
             raise ValueError("one beam list, cache and processed_frames value per stream")
@@ -864,20 +890,18 @@ class BeamSearchDecoderCTC:
                 raise ValueError("hotword_scorer_list has %d entries for %d streams" % (len(hotword_scorer_list), n))
             hot_list = [s.unigrams if s is not None else None for s in hotword_scorer_list]
             weight_list = [s.weight if s is not None else DEFAULT_HOTWORD_WEIGHT for s in hotword_scorer_list]
-        lm = self._language_model
-        starts: Optional[List[Optional[AbstractLMState]]] = None
-        if lm is not None:
-            starts = []
-            for cache in cached_lm_scores_list:
-                entry = (cache or {}).get(("", False))
-                starts.append(entry[2] if entry is not None else None)
+        # streams without a model ignore their entry (_run_locked)
+        starts: List[Optional[AbstractLMState]] = []
+        for cache in cached_lm_scores_list:
+            entry = (cache or {}).get(("", False))
+            starts.append(entry[2] if entry is not None else None)
         hot = hotword_scorer.unigrams if hotword_scorer is not None else None
         weight = hotword_scorer.weight if hotword_scorer is not None else DEFAULT_HOTWORD_WEIGHT
         mode = _lib.FIN_EOS if is_end else (_lib.FIN_FLUSH if force_next_word else _lib.FIN_KEEP)
         return self._run(logits_list, beam_width, beam_prune_logp, token_min_logp, prune_history, hot, weight,
                          max_out_beams=beam_width, lm_start_states=starts, with_state=False,
                          stream=[(list(b), int(p)) for b, p in zip(beams_list, processed_frames_list)], finalize_mode=mode,
-                         hotwords_list=hot_list, hotword_weight_list=weight_list)
+                         hotwords_list=hot_list, hotword_weight_list=weight_list, language_model_list=language_model_list)
 
     # ---- serialisation (reference decoder.py:947-1005): file plumbing only ------------------
     def save_to_dir(self, filepath: str) -> None:
