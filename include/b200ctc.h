@@ -291,6 +291,22 @@ typedef struct {
     long long single_frames;   /* one-token frames after a multi-token frame, one candidate per thread (b2c_fast_single_step) */
     int hinted;                /* 1: the beam kernel was planned from the previous call's statistics and launched without
                                   waiting for this call's (no mid-call synchronisation); same results either way */
+    int kernels;               /* one bit per beam-kernel instantiation launched by the call, the retry launch included:
+                                    bit 0  b2c_beam_fast_kernel<1024,2,64>   latency-first variant 0, V <= 64
+                                    bit 1  b2c_beam_fast_kernel<1024,2,0>    latency-first variant 0, V > 64
+                                    bit 2  b2c_beam_fast_kernel<512,3,64>    latency-first variant 1, V <= 64
+                                    bit 3  b2c_beam_fast_kernel<512,3,0>     latency-first variant 1, V > 64
+                                    bit 4  b2c_beam_fast_kernel<256,4,64>    latency-first variant 2, V <= 64
+                                    bit 5  b2c_beam_fast_kernel<256,4,0>     latency-first variant 2, V > 64
+                                    bit 6  b2c_beam_kernel<true,256,1>       capacity class 2048 / 4096
+                                    bit 7  b2c_beam_kernel<true,128,2>       capacity class 512 / 1024
+                                    bit 8  b2c_beam_kernel<true,64,4>        capacity class 256
+                                    bit 9  b2c_beam_kernel<true,32,8>        capacity class 128
+                                    bit 10 b2c_beam_kernel<false,256,1>      general kernel, one CTA per SM
+                                    bit 11 b2c_beam_kernel<false,512,1>      general kernel, beam tables in HBM
+                                    bit 12 b2c_beam_kernel<false,128,2>      general kernel, two CTAs per SM */
+    int retried;               /* utterances whose first-pass arenas overflowed and that the general kernel decoded again
+                                  with worst-case arenas (their results are those of the second decode) */
 } b2c_timings_t;
 int b2c_decoder_last_timings(const b2c_decoder_t* dec, b2c_timings_t* out);
 /* Diagnostics: the (token id, log-prob) lists the streaming stage wrote in the LAST call, as the beam kernel consumed

@@ -95,6 +95,8 @@ class Timings(C.Structure):
         ("sorted_frames", C.c_longlong),
         ("single_frames", C.c_longlong),
         ("hinted", C.c_int),
+        ("kernels", C.c_int),
+        ("retried", C.c_int),
     ]
 
 

@@ -70,8 +70,10 @@ static u32 pow2_ge(u32 x) {
 // HBM tier, beam tables in shared memory (the caller checks smem_bytes against the budget).
 // cap_request == 0: general layout -- what fits in shared memory plus an HBM tier sized for the
 // worst case beam_width * V.
+// text_limit > 0 (B200CTC_TEXT_ARENA, tests): the text arena of a first pass (!full_caps) holds at most that many nodes
 static B2cLayout make_layout(int W, int V, int T_max, bool full_caps, u32 smem_budget, u32 cap_request, u64 worst_m = 0, int n_warps = 4,
-                             u64 extra_chain = 0, u64 extra_text = 0, int n_lm = 1, int n_bucket = B2C_NBUCKET, u32 cap_max = 512) {
+                             u64 extra_chain = 0, u64 extra_text = 0, int n_lm = 1, int n_bucket = B2C_NBUCKET, u32 cap_max = 512,
+                             u32 text_limit = 0) {
     B2cLayout L;
     std::memset(&L, 0, sizeof(L));
     L.W = W;
@@ -104,6 +106,7 @@ static B2cLayout make_layout(int W, int V, int T_max, bool full_caps, u32 smem_b
     const u64 wt = static_cast<u64>(W) * static_cast<u64>(std::max(T_max, 1));
     L.chain_cap = static_cast<u32>(std::min<u64>(wt + 16 + extra_chain, 0x7FFFFFF0ull));
     L.text_cap = static_cast<u32>(std::min<u64>((full_caps ? wt + 16 : wt / 4 + 4096) + extra_text, 0x7FFFFFF0ull));
+    if (!full_caps && text_limit) L.text_cap = std::min(L.text_cap, text_limit);
     u64 s = 0;
     L.s_sc = static_cast<u32>(s); s += 128;
     if (L.beams_in_smem) {
@@ -716,6 +719,7 @@ struct Geometry {
     size_t esz = 4;               // element size of the logits the streaming stage reads
     bool streaming = false, hint_ok = false, pipelined = false;
     u32 smem_budget = 0;
+    u32 text_limit = 0;           // > 0: text-arena nodes of a first pass at most (B200CTC_TEXT_ARENA)
     const int32_t* T = nullptr;
     const int* order = nullptr;   // utterance ids, longest first
 };
@@ -723,6 +727,8 @@ struct Geometry {
 struct Knobs {
     bool host_prof, no_pipe, no_hinted, force_v5, no_v5, pipe_all, no_gate, gate_early, no_single;
     int v5_variant, force_chunks;  // v5_variant -1: chosen from the hint
+    int force_class;               // -1: planned; 0..kNumCaps-1: that capacity class; kNumCaps: the general kernel; -2: bad value
+    u32 text_arena;                // 0: default text arenas; n: a first pass gets at most n nodes
 };
 static bool env_set(const char* name) { return std::getenv(name) != nullptr; }
 static Knobs read_knobs() {
@@ -738,6 +744,17 @@ static Knobs read_knobs() {
     k.pipe_all = env_set("B200CTC_PIPELINE_ALL"); k.no_gate = env_set("B200CTC_NO_GATE");
     k.gate_early = env_set("B200CTC_HOSTSIM_GATE_EARLY");  // hostsim tests: the later chunks of a gated launch never arrive
     k.no_single = env_set("B200CTC_NO_SINGLE_STEP");       // tests: one-token frames after multi-token frames take the general step
+    // tests: every utterance the capacity-class kernels may take goes to class <0..5>, or every utterance to the general
+    // kernel ("general"); no latency-first kernel, no hint, no residency upgrade.  Each class is exact (frames wider than
+    // its shared-memory tier take the HBM-tier step), so this picks code, never results.
+    const char* cl = std::getenv("B200CTC_FORCE_CLASS");
+    k.force_class = -1;
+    if (cl && *cl) k.force_class = std::strcmp(cl, "general") == 0 ? kNumCaps : (cl[0] >= '0' && cl[0] < '0' + kNumCaps && !cl[1]) ? cl[0] - '0' : -2;
+    // tests: the text arena of a first pass holds at most n nodes, so that word commits overflow it and the retry pass
+    // runs.  At least 1: b2c_utt_begin writes the root (node 0, and its MultiLanguageModel states) without a capacity
+    // check; every other node goes through b2c_commit_text, which checks.
+    const char* ta = std::getenv("B200CTC_TEXT_ARENA");
+    k.text_arena = (ta && *ta) ? static_cast<u32>(std::max(1ll, std::min(std::atoll(ta), 0x7FFFFFF0ll))) : 0u;
     return k;
 }
 struct Plan {
@@ -748,6 +765,7 @@ struct Plan {
     std::vector<int> bounds;      // chunk boundaries along T ({0, T_max}: one chunk)
     bool gated = false;           // chunks feed ONE beam launch through device flags
     bool redo_plain = false;      // a pipelined call that cannot be planned as one: redo it as a plain call
+    bool bad_class = false;       // B200CTC_FORCE_CLASS names a class whose layout does not fit shared memory
 };
 
 // the metadata block, pinned on the host and mirrored on the device: [n] frame offsets (at 0), [n] T, [n + 1] run offsets
@@ -828,7 +846,7 @@ struct Call {
     Call(const b2c_decoder* d, const void* const* lg, const int32_t* t, int n, int dtype, int dev, const b2c_decode_opts_t* o, bool pipe)
         : logits(lg), T(t), opts(o), dtype_in(dtype), half_in(dtype == B2C_DTYPE_F16 || dtype == B2C_DTYPE_BF16), f64(dtype == B2C_DTYPE_F64),
           is_device(dev != 0), allow_pipe(pipe), esz_in(half_in ? 2 : (f64 ? 8 : 4)), k(read_knobs()) {
-        g.n_utts = n; g.V = d->V; g.beam_width = o->beam_width; g.esz = f64 ? 8 : 4; g.T = t;
+        g.n_utts = n; g.V = d->V; g.beam_width = o->beam_width; g.esz = f64 ? 8 : 4; g.T = t; g.text_limit = k.text_arena;
         std::memset(&P, 0, sizeof(P)); std::memset(&PA, 0, sizeof(PA)); std::memset(&BA, 0, sizeof(BA));
     }
     int* h_ord() const { return reinterpret_cast<int*>(hm + meta.ord); }
@@ -914,11 +932,20 @@ static int launch_gather(b2c_decoder* d, const Call& c) {
 #endif
 }
 
+// the bit of b2c_timings_t.kernels (include/b200ctc.h) of the instantiation that the CUDA branch of launch_beam below
+// dispatches a launch to; hostsim reports the same bit for the same plan
+static int kernel_bit(const Launch& ln, int V) {
+    if (ln.v5 >= 0) return 2 * ln.v5 + (V <= B2C_FAST_LT ? 0 : 1);
+    if (ln.cls < kNumCaps) return ln.threads == 32 ? 9 : ln.threads == 256 ? 6 : ln.threads == 64 ? 8 : 7;
+    return ln.threads == 512 ? 11 : ln.threads == 256 ? 10 : 12;
+}
+
 // one beam launch; `record`: its shape goes into the timings (cap_candidates, cta_threads, cta_slots, kernel_variant)
 static int launch_beam(b2c_decoder* d, const B2cBeamArgs& A, const Launch& ln, cudaStream_t stream, bool record) {
     const int slots = ln.slots, v5 = ln.v5, threads = ln.threads;
     const bool fast = ln.cls < kNumCaps;
     d->tm.launches += 1;
+    d->tm.kernels |= 1 << kernel_bit(ln, A.P.V);
     if (record) {
         d->tm.cap_candidates = static_cast<int>(ln.L.cap_s); d->tm.cta_threads = threads; d->tm.cta_slots = slots;
         d->tm.kernel_variant = v5 >= 0 ? 2 : (fast ? 1 : 0);
@@ -979,11 +1006,11 @@ static int launch_beam(b2c_decoder* d, const B2cBeamArgs& A, const Launch& ln, c
 static B2cLayout class_layout(const Geometry& g, int c, int tmax, bool full, u64 worst_m) {
     // the 2048 / 4096-candidate classes own an SM anyway: they rank over the wide bucket array
     return make_layout(g.beam_width, g.V, tmax, full, g.smem_budget, kCaps[c], worst_m, threads_of(c) / 32, 0, 0, 1,
-                       kCaps[c] >= 2048 ? B2C_NBUCKET_WIDE : B2C_NBUCKET);
+                       kCaps[c] >= 2048 ? B2C_NBUCKET_WIDE : B2C_NBUCKET, 512, g.text_limit);
 }
 static B2cLayout general_layout(const Geometry& g, int tmax, bool full, u64 worst_m, u32 cap_max) {
     return make_layout(g.W_tab, g.V, tmax, full, g.smem_budget, 0, worst_m, B2C_MAXWARPS, static_cast<u64>(g.s_max_beams),
-                       g.s_max_words + static_cast<u64>(g.s_max_beams), g.n_lm, B2C_NBUCKET_WIDE, cap_max);
+                       g.s_max_words + static_cast<u64>(g.s_max_beams), g.n_lm, B2C_NBUCKET_WIDE, cap_max, g.text_limit);
 }
 
 // the launch over `utts` in class cls (kNumCaps: the general kernel); full: worst-case arenas
@@ -1005,7 +1032,7 @@ static Launch plan_launch(const Geometry& g, const u32* maxk, const Plan& p, int
         ln.threads = B2C_FAST_WC;
         // backtrack arena: fixed node ids of the frame steps below B2C_FAST_WC * T, the out-of-line step allocates above
         ln.L = make_layout(B2C_FAST_WC, g.V, tmax, full, g.smem_budget, cap5, std::max<u64>(worst_m, cap5 + 1), B2C_FAST_NW,
-                           static_cast<u64>(B2C_FAST_WC) * static_cast<u64>(std::max(tmax, 1)));
+                           static_cast<u64>(B2C_FAST_WC) * static_cast<u64>(std::max(tmax, 1)), 0, 1, B2C_NBUCKET, 512, g.text_limit);
         ln.L.smem_bytes = static_cast<u32>(kV5Smem[ln.v5][g.V <= B2C_FAST_LT ? 1 : 0]);
         ln.per_sm = kV5Occ[ln.v5];
     } else {
@@ -1097,15 +1124,18 @@ static Plan make_plan(const Geometry& g, const u32* maxk, const u32* sumk, const
     for (int c = 0; c < kNumCaps; ++c) cap_ok[c] = class_layout(g, c, 1, false, 0).smem_bytes <= g.smem_budget;
     std::vector<int> cls_of(g.n_utts, kNumCaps);
     int top = -1, n_fast = 0;
+    const bool forced = k.force_class >= 0;     // B200CTC_FORCE_CLASS: one class (or the general kernel) for every utterance
     for (int u = 0; u < g.n_utts; ++u) {
         const double mean_k = g.T[u] > 0 ? static_cast<double>(sumk[u]) / g.T[u] : 1.0;
         const u32 typ_k = std::min<u32>(std::max<u32>(maxk[u], 1u), std::max<u32>(4u, static_cast<u32>(std::ceil(2.5 * mean_k))));
         const u64 need = std::min<u64>(static_cast<u64>(g.beam_width) * typ_k, static_cast<u64>(g.beam_width) * static_cast<u64>(g.V));
         for (int c = 0; c < kNumCaps && !g.streaming && g.n_lm == 1; ++c)      // streaming / multi-LM calls take the general kernel
             if (cap_ok[c] && need <= kCaps[c]) { cls_of[u] = c; break; }
+        if (forced && !g.streaming && g.n_lm == 1) cls_of[u] = k.force_class;
         if (cls_of[u] < kNumCaps) { top = std::max(top, cls_of[u]); ++n_fast; }
     }
-    if (top >= 0 && g.hint_ok) {
+    p.bad_class = forced && k.force_class < kNumCaps && !cap_ok[k.force_class];
+    if (top >= 0 && g.hint_ok && !forced) {
         int c_hint = kNumCaps - 1;
         for (int c = 0; c < kNumCaps; ++c)
             if (static_cast<double>(d.hint_over[c]) <= 0.004 * d.hint_frames) { c_hint = c; break; }
@@ -1114,14 +1144,14 @@ static Plan make_plan(const Geometry& g, const u32* maxk, const u32* sumk, const
     }
     const int v5_top = top;                    // the class the statistics ask for, before the residency upgrade
     // upgrade while every fast utterance stays resident (fewer frames need the out-of-line step)
-    while (top >= 0 && top + 1 < kNumCaps && cap_ok[top + 1]) {
+    while (!forced && top >= 0 && top + 1 < kNumCaps && cap_ok[top + 1]) {
         const u32 sb = class_layout(g, top + 1, 1, false, 0).smem_bytes;
         if (static_cast<long long>(d.n_sm) * per_sm_of(sb, threads_of(top + 1)) < n_fast) break;
         ++top;
     }
     // beam_width <= 128 and a typical frame within 1024 candidates: the latency-first kernel (v5) takes
     // the whole fast list; wider frames inside it go through its out-of-line HBM-tier step
-    p.use_v5 = top >= 0 && g.beam_width <= 128 && (k.force_v5 || kCaps[v5_top >= 0 ? v5_top : top] <= 1024) &&
+    p.use_v5 = !forced && top >= 0 && g.beam_width <= 128 && (k.force_v5 || kCaps[v5_top >= 0 ? v5_top : top] <= 1024) &&
                kV5Smem[0][1] + 1024 <= d.smem_optin && !k.no_v5;
     // more utterances than variant A keeps resident: trade capacity for residency if the previous call's
     // histogram says that all but 0.4% of the frames fit (hint_over[q] = frames with > 128 << q candidates)
@@ -1908,6 +1938,9 @@ static int plan_call(b2c_decoder* d, Call& c) {
         c.maxk = d->h_maxk.as<u32>();
         c.plan = make_plan(g, c.maxk, d->h_sumk.as<u32>(), *d, c.k);
     }
+    if (c.k.force_class == -2) return fail(B2C_E_ARG, "B200CTC_FORCE_CLASS must be a capacity class 0..5 or \"general\"");
+    if (c.plan.bad_class)
+        return fail(B2C_E_ARG, "B200CTC_FORCE_CLASS=" + std::to_string(c.k.force_class) + ": the layout of that class does not fit shared memory");
     d->tm.hinted = c.hinted ? 1 : 0;
     u32* h_next = reinterpret_cast<u32*>(c.hm + c.meta.next);
     for (size_t i = 0; i < 16; ++i) h_next[i] = 0;
@@ -2086,6 +2119,7 @@ static int retry_failed(b2c_decoder* d, Call& c) {
     std::vector<int> failed;
     for (int i = 0; i < n; ++i) if (status[i] != B2C_OK) failed.push_back(i);
     if (failed.empty()) return 0;
+    d->tm.retried = static_cast<int>(failed.size());
     const Launch ln = plan_launch(c.g, c.maxk, c.plan, d->n_sm, failed, kNumCaps, true, static_cast<size_t>(n));
     if (ln.L.smem_bytes > d->smem_optin) return fail(B2C_E_ARG, "beam_width too large for the shared-memory selection arrays");
     if (d->d_ws.ensure(static_cast<u64>(ln.slots) * ln.L.gws_bytes)) return B2C_E_NOMEM;
