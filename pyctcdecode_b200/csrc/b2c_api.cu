@@ -290,28 +290,6 @@ B2C_HD void b2c_beam_block(const B2cBeamArgs& A, int slot, u8* smem) {
 }
 
 #include "b2c_beam_fast.h"
-// latency-first kernel variants (beam_width <= 128): candidate capacity x resident CTAs per SM.  A is the
-// latency choice (batch resident at once); B and C trade capacity for residency when the batch is larger
-// than the resident set and the candidate histogram of the previous call says the frames fit.
-// Each variant exists with the label table resident in shared memory (alphabets of up to B2C_FAST_LT labels: runs of
-// in-place frames enabled) and with per-frame label staging (larger alphabets).
-#define B2C_FAST_LT 64
-typedef B2cFastSmem<1024, B2C_FAST_LT> B2cFastSmemA;      // 2 CTAs per SM
-typedef B2cFastSmem<512, B2C_FAST_LT> B2cFastSmemB;       // 3 CTAs per SM
-typedef B2cFastSmem<256, B2C_FAST_LT> B2cFastSmemC;       // 4 CTAs per SM
-static const u32 kV5Cap[3] = {1024, 512, 256};
-static const int kV5Occ[3] = {2, 3, 4};
-// [variant][0: staged labels, 1: resident table]
-static const size_t kV5Smem[3][2] = {{sizeof(B2cFastSmem<1024, 0>), sizeof(B2cFastSmemA)},
-                                     {sizeof(B2cFastSmem<512, 0>), sizeof(B2cFastSmemB)},
-                                     {sizeof(B2cFastSmem<256, 0>), sizeof(B2cFastSmemC)}};
-// bytes a CTA parks between two chunked launches: everything in front of the per-frame candidate scratch
-typedef B2cFastSmem<1024, 0> B2cFastSmemA0;
-typedef B2cFastSmem<512, 0> B2cFastSmemB0;
-typedef B2cFastSmem<256, 0> B2cFastSmemC0;
-static const size_t kV5Save[3][2] = {{offsetof(B2cFastSmemA0, ckey), offsetof(B2cFastSmemA, ckey)},
-                                     {offsetof(B2cFastSmemB0, ckey), offsetof(B2cFastSmemB, ckey)},
-                                     {offsetof(B2cFastSmemC0, ckey), offsetof(B2cFastSmemC, ckey)}};
 #define B2C_PIPE_CHUNKS 4
 static bool env_switch(const char* name, bool dflt) {
     const char* e = std::getenv(name);
@@ -319,9 +297,6 @@ static bool env_switch(const char* name, bool dflt) {
     return !(e[0] == '0' && e[1] == 0);
 }
 #define B2C_E_RETRY_PLAIN (-1000)     // internal: the pipelined attempt must be redone as a plain call
-static_assert(2 * (sizeof(B2cFastSmemA) + 1024) <= 228 * 1024, "variant A: 2 CTAs per SM");
-static_assert(3 * (sizeof(B2cFastSmemB) + 1024) <= 228 * 1024, "variant B: 3 CTAs per SM");
-static_assert(4 * (sizeof(B2cFastSmemC) + 1024) <= 228 * 1024, "variant C: 4 CTAs per SM");
 
 // half-precision logits (B2C_DTYPE_F16 / B2C_DTYPE_BF16) travel over PCIe as they are and are widened to float32 on the
 // device, exactly (every half / bfloat16 value is a float32 value); the path then computes as for float32 input
@@ -552,7 +527,7 @@ struct b2c_decoder {
     Event prep_ev[3];                     // inputs ready / first chunk streamed / all streamed and decided
     bool pipe_refused = false;            // the last pipelined attempt of this configuration could not be planned
     double last_device_ms = 0.0;          // streaming stage + beam kernel of the previous call (chunk sizing of pipelined calls)
-    int plain_v5 = -2, plain_cap = 0;     // kernel variant / capacity class of the last PLAIN call (pipelined calls must plan the same)
+    struct { int row = -1; u32 cap = 0; } plain;   // kBeamKernels row (-1: none) and capacity of the last PLAIN call's launch
     // hinted plain calls: the beam kernel is planned from the hint alone and launched right behind the streaming stage
     // (no wait for this call's token statistics in the middle of the call) when that plan is the one the last
     // statistics-based call of the configuration ran
@@ -702,16 +677,87 @@ static void assemble_beam(const b2c_decoder* d, const u32* toks, int nt, const i
 // capacity classes of the shared-memory candidate tier
 static const int kNumCaps = 6;
 static const u32 kCaps[kNumCaps] = {128, 256, 512, 1024, 2048, 4096};
+enum { kGeneral = 0, kClass = 1, kLatencyFirst = 2 };   // family of a beam-kernel instantiation: b2c_timings_t.kernel_variant
+#ifdef B2C_HOSTSIM
+typedef void (*BeamLauncher)(const B2cBeamArgs& A, int slot, u8* smem);   // the block function, run CTA by CTA
+template <int CAP, int OCC, int LT> constexpr BeamLauncher fast_launcher = b2c_beam_block_fast<CAP, LT>;
+template <bool FAST, int THREADS, int OCC> constexpr BeamLauncher beam_launcher = b2c_beam_block<FAST>;
+#else
+typedef int (*BeamLauncher)(const B2cBeamArgs& A, int slots, cudaStream_t stream);
+template <int CAP, int OCC, int LT>
+static int fast_launcher(const B2cBeamArgs& A, int slots, cudaStream_t stream) {
+    CUDA_OK(cudaFuncSetAttribute(b2c_beam_fast_kernel<CAP, OCC, LT>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(A.L.smem_bytes)));
+    b2c_beam_fast_kernel<CAP, OCC, LT><<<slots, B2C_FAST_WC, A.L.smem_bytes, stream>>>(A);
+    return 0;
+}
+template <bool FAST, int THREADS, int OCC>
+static int beam_launcher(const B2cBeamArgs& A, int slots, cudaStream_t stream) {
+    const int smem = static_cast<int>(A.L.smem_bytes);
+    if (smem > 48 * 1024)
+        CUDA_OK(cudaFuncSetAttribute(b2c_beam_kernel<FAST, THREADS, OCC>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    b2c_beam_kernel<FAST, THREADS, OCC><<<slots, THREADS, A.L.smem_bytes, stream>>>(A);
+    return 0;
+}
+#endif
+struct BeamKernel {
+    int family;
+    int threads;          // per CTA
+    int occ;              // the __launch_bounds__ occupancy: the most CTAs per SM a plan may assume
+    // latency-first rows only: candidate capacity, label-table entries (B2C_FAST_LT: the table is resident in shared
+    // memory and runs of in-place frames are enabled; 0: labels are staged per frame), dynamic shared memory, and the
+    // bytes a CTA parks between two chunked launches (everything in front of the per-frame candidate scratch)
+    u32 cap;
+    int lt;
+    size_t smem, save;
+    BeamLauncher launch;
+};
+// one row per kernel template: every number of an instantiation is written once, in its template arguments
+template <int CAP, int OCC, int LT>
+constexpr BeamKernel fast_row() {
+    typedef B2cFastSmem<CAP, LT> S;
+    static_assert(OCC * (sizeof(S) + 1024) <= 228 * 1024, "OCC CTAs of the variant fit an SM's shared memory");
+    return {kLatencyFirst, B2C_FAST_WC, OCC, CAP, LT, sizeof(S), offsetof(S, ckey), fast_launcher<CAP, OCC, LT>};
+}
+template <int THREADS, int OCC>
+constexpr BeamKernel class_row() { return {kClass, THREADS, OCC, 0, 0, 0, 0, beam_launcher<true, THREADS, OCC>}; }
+template <int THREADS, int OCC>
+constexpr BeamKernel general_row() { return {kGeneral, THREADS, OCC, 0, 0, 0, 0, beam_launcher<false, THREADS, OCC>}; }
+#define B2C_FAST_LT 64
+// row i is bit i of b2c_timings_t.kernels (the table in include/b200ctc.h)
+static constexpr BeamKernel kBeamKernels[13] = {
+    // latency-first variants (beam_width <= 128): candidate capacity x resident CTAs per SM.  Variant 0 is the latency
+    // choice (batch resident at once); 1 and 2 trade capacity for residency when the batch is larger than the resident
+    // set and the candidate histogram of the previous call says the frames fit.  Variant v is rows 2v (alphabets of up to
+    // B2C_FAST_LT labels) and 2v + 1 (larger alphabets).
+    fast_row<1024, 2, B2C_FAST_LT>(), fast_row<1024, 2, 0>(),
+    fast_row<512, 3, B2C_FAST_LT>(), fast_row<512, 3, 0>(),
+    fast_row<256, 4, B2C_FAST_LT>(), fast_row<256, 4, 0>(),
+    class_row<256, 1>(),       // 255 registers x 256 threads: the whole register file (classes 2048 / 4096)
+    class_row<128, 2>(),       // 255 registers x 128 threads: 2 CTAs per SM (classes 512 / 1024)
+    class_row<64, 4>(),        // 255 registers x 64 threads: 4 CTAs per SM (class 256)
+    class_row<32, 8>(),        // 255 registers x 32 threads: 8 one-warp CTAs per SM (class 128)
+    general_row<256, 1>(),     // one CTA per SM
+    general_row<512, 1>(),     // 128 registers x 512 threads (beam tables in HBM: latency-bound)
+    general_row<128, 2>(),     // two CTAs per SM
+};
+// the row of latency-first variant v (0..2) for an alphabet of V labels
+static int v5_row(int v, int V) { return 2 * v + (V <= B2C_FAST_LT ? 0 : 1); }
+// the capacity-class or general row with `threads` threads per CTA (the plan asks only for shapes the table has)
+static int beam_row(int family, int threads) {
+    int r = 0;
+    while (kBeamKernels[r].family != family || kBeamKernels[r].threads != threads) ++r;
+    return r;
+}
 // big classes leave room for one CTA per SM only: give that CTA 256 threads (a diffuse frame has ~650 candidates)
-static int threads_of(int c) { return kCaps[c] <= 128 ? 32 : (kCaps[c] <= 256 ? 64 : (kCaps[c] >= 2048 ? 256 : 128)); }
-static int per_sm_of(u32 smem_bytes, int threads) {
+static int class_row_of(int c) { return beam_row(kClass, kCaps[c] <= 128 ? 32 : (kCaps[c] <= 256 ? 64 : (kCaps[c] >= 2048 ? 256 : 128))); }
+static int per_sm_of(int row, u32 smem_bytes) {
     const int by_smem = static_cast<int>(std::max<u64>(1, (224 * 1024) / std::max<u32>(smem_bytes + 1024, 2048)));
-    return std::min(by_smem, threads == 32 ? 8 : (threads == 64 ? 4 : (threads >= 256 ? 1 : 2)));
+    return std::min(by_smem, kBeamKernels[row].occ);
 }
 
 // one beam launch: utterances [ord_off, ord_off + count) of the work list, capacity class cls (kNumCaps: general kernel),
-// v5 >= 0: variant of the latency-first kernel (b2c_beam_fast.h; L.smem_bytes is kV5Smem[v5] then)
-struct Launch { int cls; size_t ord_off; int count; B2cLayout L; int slots; int per_sm; int threads; int v5; };
+// run by kBeamKernels[row] (a latency-first row: L.smem_bytes is the row's smem)
+struct Launch { int cls; size_t ord_off; int count; B2cLayout L; int slots; int per_sm; int row; };
 // the shape of a call: what its launch plan is made from besides the token statistics and the decoder's hint
 struct Geometry {
     int n_utts = 0, V = 0, beam_width = 0, W_tab = 0, n_lm = 1, s_max_beams = 0, T_max = 0;
@@ -932,68 +978,21 @@ static int launch_gather(b2c_decoder* d, const Call& c) {
 #endif
 }
 
-// the bit of b2c_timings_t.kernels (include/b200ctc.h) of the instantiation that the CUDA branch of launch_beam below
-// dispatches a launch to; hostsim reports the same bit for the same plan
-static int kernel_bit(const Launch& ln, int V) {
-    if (ln.v5 >= 0) return 2 * ln.v5 + (V <= B2C_FAST_LT ? 0 : 1);
-    if (ln.cls < kNumCaps) return ln.threads == 32 ? 9 : ln.threads == 256 ? 6 : ln.threads == 64 ? 8 : 7;
-    return ln.threads == 512 ? 11 : ln.threads == 256 ? 10 : 12;
-}
-
 // one beam launch; `record`: its shape goes into the timings (cap_candidates, cta_threads, cta_slots, kernel_variant)
 static int launch_beam(b2c_decoder* d, const B2cBeamArgs& A, const Launch& ln, cudaStream_t stream, bool record) {
-    const int slots = ln.slots, v5 = ln.v5, threads = ln.threads;
-    const bool fast = ln.cls < kNumCaps;
+    const BeamKernel& k = kBeamKernels[ln.row];
     d->tm.launches += 1;
-    d->tm.kernels |= 1 << kernel_bit(ln, A.P.V);
+    d->tm.kernels |= 1 << ln.row;
     if (record) {
-        d->tm.cap_candidates = static_cast<int>(ln.L.cap_s); d->tm.cta_threads = threads; d->tm.cta_slots = slots;
-        d->tm.kernel_variant = v5 >= 0 ? 2 : (fast ? 1 : 0);
+        d->tm.cap_candidates = static_cast<int>(ln.L.cap_s); d->tm.cta_threads = k.threads; d->tm.cta_slots = ln.slots;
+        d->tm.kernel_variant = k.family;
     }
 #ifdef B2C_HOSTSIM
     (void)stream;
     std::vector<u8> smem(A.L.smem_bytes + 64);
-    const bool table = A.P.V <= B2C_FAST_LT;
-    for (int s = 0; s < slots; ++s) {
-        if (v5 == 0) table ? b2c_beam_block_fast<1024, B2C_FAST_LT>(A, s, smem.data()) : b2c_beam_block_fast<1024, 0>(A, s, smem.data());
-        else if (v5 == 1) table ? b2c_beam_block_fast<512, B2C_FAST_LT>(A, s, smem.data()) : b2c_beam_block_fast<512, 0>(A, s, smem.data());
-        else if (v5 == 2) table ? b2c_beam_block_fast<256, B2C_FAST_LT>(A, s, smem.data()) : b2c_beam_block_fast<256, 0>(A, s, smem.data());
-        else if (fast) b2c_beam_block<true>(A, s, smem.data());
-        else b2c_beam_block<false>(A, s, smem.data());
-    }
+    for (int s = 0; s < ln.slots; ++s) k.launch(A, s, smem.data());
 #else
-    const int smem = static_cast<int>(A.L.smem_bytes);
-#define B2C_LAUNCH_V5(CAP, OCC, LT)                                                                                     \
-    do {                                                                                                               \
-        CUDA_OK(cudaFuncSetAttribute(b2c_beam_fast_kernel<CAP, OCC, LT>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)); \
-        b2c_beam_fast_kernel<CAP, OCC, LT><<<slots, B2C_FAST_WC, A.L.smem_bytes, stream>>>(A);                        \
-    } while (0)
-    if (v5 >= 0) {
-        const bool table = A.P.V <= B2C_FAST_LT;
-        if (v5 == 0 && table) B2C_LAUNCH_V5(1024, 2, B2C_FAST_LT);
-        else if (v5 == 0) B2C_LAUNCH_V5(1024, 2, 0);
-        else if (v5 == 1 && table) B2C_LAUNCH_V5(512, 3, B2C_FAST_LT);
-        else if (v5 == 1) B2C_LAUNCH_V5(512, 3, 0);
-        else if (table) B2C_LAUNCH_V5(256, 4, B2C_FAST_LT);
-        else B2C_LAUNCH_V5(256, 4, 0);
-        CUDA_OK(cudaGetLastError());
-        return 0;
-    }
-#undef B2C_LAUNCH_V5
-#define B2C_LAUNCH_BEAM(FAST, THREADS, OCC)                                                                            \
-    do {                                                                                                               \
-        if (smem > 48 * 1024)                                                                                          \
-            CUDA_OK(cudaFuncSetAttribute(b2c_beam_kernel<FAST, THREADS, OCC>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)); \
-        b2c_beam_kernel<FAST, THREADS, OCC><<<slots, THREADS, A.L.smem_bytes, stream>>>(A);                           \
-    } while (0)
-    if (fast && threads == 32) B2C_LAUNCH_BEAM(true, 32, 8);           // 255 registers x 32 threads: 8 one-warp CTAs per SM
-    else if (fast && threads == 256) B2C_LAUNCH_BEAM(true, 256, 1);    // 255 registers x 256 threads: the whole register file
-    else if (fast && threads == 64) B2C_LAUNCH_BEAM(true, 64, 4);     // 255 registers x 64 threads: 4 CTAs per SM
-    else if (fast) B2C_LAUNCH_BEAM(true, 128, 2);                 // 255 registers x 128 threads: 2 CTAs per SM
-    else if (threads == 512) B2C_LAUNCH_BEAM(false, 512, 1);      // 128 registers x 512 threads (beam tables in HBM: latency-bound)
-    else if (threads == 256) B2C_LAUNCH_BEAM(false, 256, 1);
-    else B2C_LAUNCH_BEAM(false, 128, 2);
-#undef B2C_LAUNCH_BEAM
+    B2C_TRY(k.launch(A, ln.slots, stream));
     CUDA_OK(cudaGetLastError());
 #endif
     return 0;
@@ -1005,7 +1004,7 @@ static int launch_beam(b2c_decoder* d, const B2cBeamArgs& A, const Launch& ln, c
 // =========================================================================================
 static B2cLayout class_layout(const Geometry& g, int c, int tmax, bool full, u64 worst_m) {
     // the 2048 / 4096-candidate classes own an SM anyway: they rank over the wide bucket array
-    return make_layout(g.beam_width, g.V, tmax, full, g.smem_budget, kCaps[c], worst_m, threads_of(c) / 32, 0, 0, 1,
+    return make_layout(g.beam_width, g.V, tmax, full, g.smem_budget, kCaps[c], worst_m, kBeamKernels[class_row_of(c)].threads / 32, 0, 0, 1,
                        kCaps[c] >= 2048 ? B2C_NBUCKET_WIDE : B2C_NBUCKET, 512, g.text_limit);
 }
 static B2cLayout general_layout(const Geometry& g, int tmax, bool full, u64 worst_m, u32 cap_max) {
@@ -1025,37 +1024,36 @@ static Launch plan_launch(const Geometry& g, const u32* maxk, const Plan& p, int
         kmax = std::max(kmax, maxk[u]);
     }
     const u64 worst_m = static_cast<u64>(g.W_tab) * std::min<u32>(kmax, static_cast<u32>(g.V));
-    ln.v5 = (p.use_v5 && cls < kNumCaps) ? p.v5_variant : -1;
-    if (ln.v5 >= 0) {
+    if (p.use_v5 && cls < kNumCaps) {
+        ln.row = v5_row(p.v5_variant, g.V);
+        const BeamKernel& k = kBeamKernels[ln.row];
         // beam tables of capacity 128; the HBM tier always exists (frames with more tokens than the rings hold use it too)
-        const u32 cap5 = kV5Cap[ln.v5];
-        ln.threads = B2C_FAST_WC;
         // backtrack arena: fixed node ids of the frame steps below B2C_FAST_WC * T, the out-of-line step allocates above
-        ln.L = make_layout(B2C_FAST_WC, g.V, tmax, full, g.smem_budget, cap5, std::max<u64>(worst_m, cap5 + 1), B2C_FAST_NW,
+        ln.L = make_layout(B2C_FAST_WC, g.V, tmax, full, g.smem_budget, k.cap, std::max<u64>(worst_m, k.cap + 1), B2C_FAST_NW,
                            static_cast<u64>(B2C_FAST_WC) * static_cast<u64>(std::max(tmax, 1)), 0, 1, B2C_NBUCKET, 512, g.text_limit);
-        ln.L.smem_bytes = static_cast<u32>(kV5Smem[ln.v5][g.V <= B2C_FAST_LT ? 1 : 0]);
-        ln.per_sm = kV5Occ[ln.v5];
+        ln.L.smem_bytes = static_cast<u32>(k.smem);
+        ln.per_sm = k.occ;
     } else {
-        ln.threads = cls < kNumCaps ? threads_of(cls) : 128;
         if (cls < kNumCaps) {
+            ln.row = class_row_of(cls);
             ln.L = class_layout(g, cls, tmax, full, worst_m);
         } else {
             // general kernel: the largest shared-memory candidate tier that fits (frames beyond it work on the HBM tier at
             // L2 latency) -- unless the launch has more utterances than SMs and the small tier keeps two CTAs per SM
+            const int r128 = beam_row(kGeneral, 128);
             ln.L = general_layout(g, tmax, full, worst_m, 2048);
-            if (per_sm_of(ln.L.smem_bytes, 128) == 1 && ln.count > n_sm) {
+            if (per_sm_of(r128, ln.L.smem_bytes) == 1 && ln.count > n_sm) {
                 const B2cLayout small = general_layout(g, tmax, full, worst_m, 512);
-                if (per_sm_of(small.smem_bytes, 128) >= 2) ln.L = small;
+                if (per_sm_of(r128, small.smem_bytes) >= 2) ln.L = small;
             }
+            // room for one CTA per SM only (wide beams): that CTA gets the whole register file -- its phases are loops over
+            // hundreds to thousands of candidates, each a chain of dependent memory accesses.  Beam tables that do not fit
+            // shared memory (beam_width in the thousands) live in HBM: every phase is a chain of L2 round trips, and twice
+            // the threads at half the registers hide more of them (with the tables in shared memory, e.g. beam 500, the
+            // spills cost more than they hide)
+            ln.row = per_sm_of(r128, ln.L.smem_bytes) > 1 ? r128 : beam_row(kGeneral, ln.L.beams_in_smem ? 256 : 512);
         }
-        // the general kernel with room for one CTA per SM only (wide beams): that CTA gets the whole register file --
-        // its phases are loops over hundreds to thousands of candidates, each a chain of dependent memory accesses
-        if (cls == kNumCaps && per_sm_of(ln.L.smem_bytes, 128) == 1) ln.threads = 256;
-        // beam tables that do not fit shared memory (beam_width in the thousands) live in HBM: every phase is a chain of L2
-        // round trips, and twice the threads at half the registers hide more of them (with the tables in shared memory,
-        // e.g. beam 500, the spills cost more than they hide)
-        if (cls == kNumCaps && ln.threads == 256 && !ln.L.beams_in_smem) ln.threads = 512;
-        ln.per_sm = per_sm_of(ln.L.smem_bytes, ln.threads);
+        ln.per_sm = per_sm_of(ln.row, ln.L.smem_bytes);
     }
     ln.slots = std::min(ln.count, n_sm * ln.per_sm);
     const u64 budget = 16ull << 30;            // keep the HBM workspace bounded
@@ -1078,19 +1076,20 @@ static Launch plan_launch(const Geometry& g, const u32* maxk, const Plan& p, int
 // The plan of a pipelined call comes from the hint alone; it must be the plan the previous plain call of this
 // configuration ran (another kernel variant would change the speed, not the result: diffuse batches decode 35 % slower
 // on the latency-first kernel the hint-only plan picks than on the capacity-class kernel their statistics pick).
+// Is `ln` the launch the last plain call ran?  (V is fixed per decoder: the row names the variant.)
+static bool ran_last_plain(const b2c_decoder& d, const Launch& ln) { return ln.row == d.plain.row && ln.L.cap_s == d.plain.cap; }
 static void plan_chunks(const Geometry& g, const b2c_decoder& d, const Knobs& k, Plan& p) {
     const int T_max = g.T_max;
     p.bounds = {0, std::max(T_max, 0)};
     // chunked launches need ONE launch of the latency-first kernel with every utterance resident
     const Launch& l0 = p.launches[0];
-    const bool can_chunk = p.launches.size() == 1 && l0.v5 >= 0 && l0.count <= l0.slots && !g.streaming;
+    const bool can_chunk = p.launches.size() == 1 && kBeamKernels[l0.row].family == kLatencyFirst && l0.count <= l0.slots && !g.streaming;
     if (g.pipelined && !can_chunk) { p.redo_plain = true; return; }
     const double copy_ms_est = static_cast<double>(g.total_frames) * g.V * g.esz / 50.0e6;            // ~50 GB/s pinned H2D
     const double r = copy_ms_est / std::max(d.last_device_ms > 0 ? d.last_device_ms : copy_ms_est, 1e-3);
     p.gated = g.pipelined && !k.no_gate && (r < 0.6 || k.pipe_all) && l0.count + d.n_sm / 8 <= d.n_sm * l0.per_sm;
     if (g.pipelined) {
-        const bool same_plan = l0.v5 == d.plain_v5 && static_cast<int>(l0.L.cap_s) == d.plain_cap;
-        if ((!p.gated && r < 0.6 && !k.pipe_all) || (!same_plan && !k.pipe_all)) { p.redo_plain = true; return; }
+        if ((!p.gated && r < 0.6 && !k.pipe_all) || (!ran_last_plain(d, l0) && !k.pipe_all)) { p.redo_plain = true; return; }
         p.bounds = {0};
         if (!p.gated && r < 0.6) {
             int f = static_cast<int>(1.15 * T_max * r / (1.0 + r));
@@ -1146,18 +1145,18 @@ static Plan make_plan(const Geometry& g, const u32* maxk, const u32* sumk, const
     // upgrade while every fast utterance stays resident (fewer frames need the out-of-line step)
     while (!forced && top >= 0 && top + 1 < kNumCaps && cap_ok[top + 1]) {
         const u32 sb = class_layout(g, top + 1, 1, false, 0).smem_bytes;
-        if (static_cast<long long>(d.n_sm) * per_sm_of(sb, threads_of(top + 1)) < n_fast) break;
+        if (static_cast<long long>(d.n_sm) * per_sm_of(class_row_of(top + 1), sb) < n_fast) break;
         ++top;
     }
     // beam_width <= 128 and a typical frame within 1024 candidates: the latency-first kernel (v5) takes
     // the whole fast list; wider frames inside it go through its out-of-line HBM-tier step
     p.use_v5 = !forced && top >= 0 && g.beam_width <= 128 && (k.force_v5 || kCaps[v5_top >= 0 ? v5_top : top] <= 1024) &&
-               kV5Smem[0][1] + 1024 <= d.smem_optin && !k.no_v5;
-    // more utterances than variant A keeps resident: trade capacity for residency if the previous call's
+               kBeamKernels[0].smem + 1024 <= d.smem_optin && !k.no_v5;
+    // more utterances than variant 0 keeps resident: trade capacity for residency if the previous call's
     // histogram says that all but 0.4% of the frames fit (hint_over[q] = frames with > 128 << q candidates)
-    if (p.use_v5 && g.hint_ok && n_fast > d.n_sm * kV5Occ[0] && k.v5_variant < 0) {
+    if (p.use_v5 && g.hint_ok && n_fast > d.n_sm * kBeamKernels[0].occ && k.v5_variant < 0) {
         for (int v = 2; v >= 1; --v) {
-            const int q = kV5Cap[v] == 256 ? 1 : 2;
+            const int q = kBeamKernels[v5_row(v, g.V)].cap == 256 ? 1 : 2;
             if (static_cast<double>(d.hint_over[q]) <= 0.004 * d.hint_frames) { p.v5_variant = v; break; }
         }
     }
@@ -1886,7 +1885,8 @@ static int run_streaming_stage(b2c_decoder* d, Call& c) {
     CUDA_OK(cudaMemcpyAsync(d->h_sumk.p, d->d_sumk.p, 4ull * n, cudaMemcpyDeviceToHost, st));
     c.hp.mark(0);                                 // argument checks, buffers, enqueue of H2D + prepare kernels
     // if the plan is not the one the last statistics-based call ran, a hinted call waits for the statistics after all
-    c.hinted = c.allow_pipe && !c.k.no_hinted && g.hint_ok && !g.streaming && g.n_lm == 1 && g.beam_width <= 128 && d->plain_v5 >= 0 &&
+    c.hinted = c.allow_pipe && !c.k.no_hinted && g.hint_ok && !g.streaming && g.n_lm == 1 && g.beam_width <= 128 &&
+               d->plain.row >= 0 && kBeamKernels[d->plain.row].family == kLatencyFirst &&
                (d->hinted_calls++ % 32u) != 31u && !d->hinted_refused;
     if ((d->hinted_calls % 32u) == 0u) d->hinted_refused = false;       // the refresh call ran: try the hint again
     if (!c.hinted) {
@@ -1928,8 +1928,7 @@ static int plan_call(b2c_decoder* d, Call& c) {
     c.maxk = nostat ? c.nostat_maxk.data() : d->h_maxk.as<u32>();
     c.plan = make_plan(g, c.maxk, nostat ? c.nostat_sumk.data() : d->h_sumk.as<u32>(), *d, c.k);
     const std::vector<Launch>& ls = c.plan.launches;
-    if (c.hinted && !(ls.size() == 1 && ls[0].v5 == d->plain_v5 && static_cast<int>(ls[0].L.cap_s) == d->plain_cap &&
-                      ls[0].slots == std::min(ls[0].count, d->n_sm * ls[0].per_sm))) {
+    if (c.hinted && !(ls.size() == 1 && ran_last_plain(*d, ls[0]) && ls[0].slots == std::min(ls[0].count, d->n_sm * ls[0].per_sm))) {
         // not the plan the last statistics-based call ran -- or the worst-case workspace of a plan without statistics (V tokens
         // in a frame: large alphabets) would cost resident CTAs: wait for this call's statistics and plan from them
         c.hinted = false; d->hinted_refused = true;
@@ -1956,7 +1955,7 @@ static int plan_call(b2c_decoder* d, Call& c) {
     if (d->d_ws.ensure(ws_need)) return B2C_E_NOMEM;
     if (c.plan.redo_plain) { d->pipe_refused = true; return B2C_E_RETRY_PLAIN; }   // until the configuration (hint) changes
     // a plain call remembers its plan: pipelined and hinted calls of the configuration must plan the same
-    if (!g.pipelined && !c.hinted && ls.size() == 1 && c.plan.bounds.size() == 2) { d->plain_v5 = ls[0].v5; d->plain_cap = static_cast<int>(ls[0].L.cap_s); }
+    if (!g.pipelined && !c.hinted && ls.size() == 1 && c.plan.bounds.size() == 2) d->plain = {ls[0].row, ls[0].L.cap_s};
     return 0;
 }
 
@@ -1972,7 +1971,7 @@ static int enqueue_chunked(b2c_decoder* d, Call& c) {
     const size_t esz = c.g.esz;
     cudaStream_t st = d->stream;
     B2cBeamArgs& BA = c.BA;
-    const u64 stride = (kV5Save[ln.v5][V <= B2C_FAST_LT ? 1 : 0] + 16 + 255) & ~255ull;
+    const u64 stride = (kBeamKernels[ln.row].save + 16 + 255) & ~255ull;
     if (d->d_state.ensure(stride * static_cast<u64>(ln.slots))) return B2C_E_NOMEM;
     BA.L = ln.L; BA.n_utts = ln.count; BA.order = c.d_ord() + ln.ord_off; BA.next = c.d_next(); BA.gws = d->d_ws.as<u8>();
     BA.state = d->d_state.as<u8>(); BA.state_stride = stride;
