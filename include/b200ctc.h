@@ -193,6 +193,12 @@ typedef struct {
      * must equal the number of models of the call's largest set (at least 1), else B2C_E_ARG (the library cannot see
      * the extent of the array).  Not read without utt_lm_set. */
     int lm_start_width;
+    /* per-utterance finalize modes: NULL, or [n_utts] B2C_FIN_* values; utterance i then ends its call as a call of its
+     * own with finalize_mode = utt_finalize_mode[i] (batched streaming where some streams end, some flush their partial
+     * words and the rest keep them), and finalize_mode is not read.  B2C_E_ARG: a value outside [B2C_FIN_EOS,
+     * B2C_FIN_KEEP], or finalize_mode != B2C_FIN_EOS together with utt_finalize_mode.  The call is a streaming call
+     * when stream_states is given or some utterance's mode is not B2C_FIN_EOS. */
+    const int32_t* utt_finalize_mode;
 } b2c_decode_opts_t;
 void b2c_decode_opts_default(b2c_decode_opts_t* opts);
 

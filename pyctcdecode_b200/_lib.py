@@ -63,6 +63,7 @@ class DecodeOpts(C.Structure):
         ("n_lm_sets", C.c_int),
         ("utt_lm_set", C.POINTER(C.c_int32)),
         ("lm_start_width", C.c_int),
+        ("utt_finalize_mode", C.POINTER(C.c_int32)),
     ]
 
 

@@ -147,7 +147,7 @@ struct B2cBeamArgs {
     u8* gws;                   // [slots][L.gws_bytes]
     const B2cLmState* start_states;  // optional [n_utts]
     // streaming calls (general kernel only): input beams per utterance, what to do at the end of the call
-    const B2cStreamUtt* s_utts;      // optional [n_utts]
+    const B2cStreamUtt* s_utts;      // optional [n_utts]; when given, its fin_mode replaces fin_mode below
     const B2cStreamBeam* s_beams;
     const u64* s_word_hash;
     const u32* s_word_len;
@@ -272,7 +272,7 @@ B2C_HD void b2c_beam_block(const B2cBeamArgs& A, int slot, u8* smem) {
         O.states = A.out_states + static_cast<u64>(u) * ob;
         O.aux = A.out_aux ? A.out_aux + 4 * static_cast<u64>(u) * ob : nullptr;
         O.states_x = A.out_states_x ? A.out_states_x + static_cast<u64>(u) * ob * A.P.lm_x : nullptr;
-        b2c_finalize(A.P, W, O, A.fin_mode);
+        b2c_finalize(A.P, W, O, A.s_utts ? A.s_utts[u].fin_mode : A.fin_mode);
         B2C_MARK(8);
     }
     B2C_LEADER {
@@ -1488,19 +1488,30 @@ static int set_geometry(Call& c) {
     return 0;
 }
 
-// streaming input (partial_decode_beams): flatten the per-utterance beam / word lists
+// streaming input (partial_decode_beams): flatten the per-utterance beam / word lists and finalize modes.  Every
+// utterance of a streaming call gets a B2cStreamUtt record (zero input beams without stream_states): it carries the
+// utterance's finalize mode to the kernel.
 static int flatten_stream_states(const b2c_decoder* d, Call& c) {
     const b2c_decode_opts_t* o = c.opts;
     Geometry& g = c.g;
+    const int32_t* modes = o->utt_finalize_mode;
     if (o->finalize_mode < B2C_FIN_EOS || o->finalize_mode > B2C_FIN_KEEP) return fail(B2C_E_ARG, "bad finalize_mode");
-    g.streaming = o->stream_states != nullptr || o->finalize_mode != B2C_FIN_EOS;
+    if (modes && o->finalize_mode != B2C_FIN_EOS) return fail(B2C_E_ARG, "opts->finalize_mode and opts->utt_finalize_mode are exclusive");
+    bool any_open = o->finalize_mode != B2C_FIN_EOS;
+    for (int i = 0; modes && i < g.n_utts; ++i) {
+        if (modes[i] < B2C_FIN_EOS || modes[i] > B2C_FIN_KEEP) return fail(B2C_E_ARG, "utt_finalize_mode value out of range");
+        any_open = any_open || modes[i] != B2C_FIN_EOS;
+    }
+    g.streaming = o->stream_states != nullptr || any_open;
     c.text_only = o->text_only != 0 && !g.streaming;
-    if (o->stream_states) {
+    if (g.streaming) {
         c.s_utts.resize(g.n_utts);
         for (int i = 0; i < g.n_utts; ++i) {
+            const int mode = modes ? modes[i] : o->finalize_mode;
+            if (!o->stream_states) { c.s_utts[i] = B2cStreamUtt{0u, 0u, 0, mode}; continue; }
             const b2c_stream_state_t& ss = o->stream_states[i];
             if (ss.n_beams < 0 || ss.n_beams > 65535 || (ss.n_beams > 0 && !ss.beams)) return fail(B2C_E_ARG, "bad stream state");
-            const B2cStreamUtt su{static_cast<u32>(c.s_beams.size()), static_cast<u32>(ss.n_beams), ss.processed_frames, 0};
+            const B2cStreamUtt su{static_cast<u32>(c.s_beams.size()), static_cast<u32>(ss.n_beams), ss.processed_frames, mode};
             const u32 wbase = static_cast<u32>(c.s_wh.size());
             u64 words = 0;
             for (int b = 0; b < ss.n_beams; ++b) {

@@ -325,7 +325,7 @@ class BeamSearchDecoderCTC:
              prune_history: bool, hotwords: Optional[Iterable[str]], hotword_weight: float, max_out_beams: int,
              lm_start_states: Optional[Sequence[Optional[AbstractLMState]]] = None, with_state: bool = True,
              device: Optional[int] = None, texts_only: bool = False, lengths: Optional[Sequence[int]] = None,
-             stream: Optional[Sequence[Tuple[Sequence[Beam], int]]] = None, finalize_mode: int = _lib.FIN_EOS,
+             stream: Optional[Sequence[Tuple[Sequence[Beam], int]]] = None, finalize_mode: Union[int, List[int]] = _lib.FIN_EOS,
              hotwords_list: Optional[Sequence[Optional[Iterable[str]]]] = None,
              hotword_weight_list: Optional[Sequence[float]] = None,
              language_model_list: Optional[Sequence[Optional[AbstractLanguageModel]]] = None) -> Any:
@@ -386,7 +386,7 @@ class BeamSearchDecoderCTC:
                     device: Optional[int], torch_stream: Optional[int], beam_width: int, beam_prune_logp: float,
                     token_min_logp: float, prune_history: bool, hotwords: Optional[Iterable[str]], hotword_weight: float,
                     max_out_beams: int, lm_start_states: Optional[Sequence[Optional[AbstractLMState]]], with_state: bool,
-                    texts_only: bool, stream: Optional[Sequence[Tuple[Sequence[Beam], int]]], finalize_mode: int,
+                    texts_only: bool, stream: Optional[Sequence[Tuple[Sequence[Beam], int]]], finalize_mode: Union[int, List[int]],
                     utt_hot: Optional[List[Tuple[List[str], float]]] = None,
                     utt_lms: Optional[List[List[LanguageModel]]] = None) -> Any:
         handle = self._handle(device)
@@ -480,7 +480,14 @@ class BeamSearchDecoderCTC:
             opts.lm_start_states = C.cast(states_arr, C.POINTER(_lib.LMState))
         if stream is not None:
             opts.stream_states = C.cast(self._stream_states(handle, stream, keep_alive), C.POINTER(_lib.StreamState))
-        opts.finalize_mode = int(finalize_mode)
+        if isinstance(finalize_mode, list):      # one B2C_FIN_* per stream
+            modes = finalize_mode
+            mode_arr = (C.c_int32 * n)(*modes)
+            keep_alive.append(mode_arr)
+            opts.utt_finalize_mode = C.cast(mode_arr, C.POINTER(C.c_int32))
+        else:
+            modes = [int(finalize_mode)] * n
+            opts.finalize_mode = int(finalize_mode)
         opts.text_only = int(bool(texts_only))
         ptrs = (C.c_void_p * n)(*[m[1] for m in mats])
         Ts = (C.c_int32 * n)(*[m[2] for m in mats])
@@ -492,7 +499,7 @@ class BeamSearchDecoderCTC:
                 _lib.check(L.b2c_result_top_texts(res, C.byref(data), C.byref(size)))
                 return C.string_at(data, size.value).decode("utf-8").split("\x00")[:n]
             if stream is not None:
-                return self._stream_results(res, stream, finalize_mode)
+                return self._stream_results(res, stream, modes)
             out = self._output_beams(L, res, with_state, n_lm)
         finally:
             L.b2c_result_free(res)
@@ -758,10 +765,10 @@ class BeamSearchDecoderCTC:
                              partial_frames=pframes, logit_score=logit, lm_score=lm)
         return beam
 
-    def _stream_results(self, res: Any, stream: Sequence[Tuple[Sequence[Beam], int]], finalize_mode: int) -> List[List[LMBeam]]:
+    def _stream_results(self, res: Any, stream: Sequence[Tuple[Sequence[Beam], int]], modes: List[int]) -> List[List[LMBeam]]:
         """What the call appended (the token chain since the input beam, replayed into strings by the library; frames of
         the words finished during the call) on top of the input beams' strings -> LMBeam lists (reference
-        _finalize_beams output)."""
+        _finalize_beams output).  modes: the B2C_FIN_* of each stream."""
         L = _lib.lib()
         pk = _lib.Packed()
         _lib.check(L.b2c_result_packed(res, C.byref(pk)))
@@ -780,7 +787,6 @@ class BeamSearchDecoderCTC:
         else:
             pairs = []
         labels = self._alphabet.labels
-        keep = finalize_mode == _lib.FIN_KEEP
         table = self._word_hash
         c0, c1 = self._text_cache
         spaced = self._labels_with_space
@@ -791,6 +797,7 @@ class BeamSearchDecoderCTC:
         k = wi = 0
         for u, nb in enumerate(counts):
             roots = stream[u][0]
+            keep = modes[u] == _lib.FIN_KEEP
             beams = []
             for _ in range(nb):
                 a0 = aux[4 * k]
@@ -868,8 +875,9 @@ class BeamSearchDecoderCTC:
                                    hotword_scorer: Optional[HotwordScorer] = None, force_next_word: bool = False,
                                    is_end: bool = False,
                                    hotword_scorer_list: Optional[Sequence[Optional[HotwordScorer]]] = None,
-                                   language_model_list: Optional[Sequence[Optional[AbstractLanguageModel]]] = None
-                                   ) -> List[List[LMBeam]]:
+                                   language_model_list: Optional[Sequence[Optional[AbstractLanguageModel]]] = None,
+                                   is_end_list: Optional[Sequence[bool]] = None,
+                                   force_next_word_list: Optional[Sequence[bool]] = None) -> List[List[LMBeam]]:
         """Extension: many independent streams advance by one chunk each in ONE kernel launch.  `hotword_scorer_list`:
         one HotwordScorer (or None) per stream instead of one `hotword_scorer` for all.
 
@@ -878,10 +886,21 @@ class BeamSearchDecoderCTC:
         returns for it.  The words its beams carry are replayed through the model of this call, so a stream may change
         its model between calls.  Its start state is read from its cache under ("", False): a MultiLanguageModelState
         of k states for a set of k models, a B200LMState for one; get_starting_state(language_model=...) makes it, and
-        a missing entry means that model's default start state."""
+        a missing entry means that model's default start state.
+
+        `is_end_list` / `force_next_word_list`: one flag per stream instead of `is_end` / `force_next_word` for all, so
+        that streams that end, streams that flush their partial word and streams that go on share one call.  Stream i
+        then gets what ``partial_decode_beams(..., force_next_word=force_next_word_list[i], is_end=is_end_list[i])``
+        returns for it."""
         n = len(logits_list)
         if not (len(beams_list) == len(processed_frames_list) == len(cached_lm_scores_list) == n):
             raise ValueError("one beam list, cache and processed_frames value per stream")
+        for name, flag, flags in (("is_end", is_end, is_end_list), ("force_next_word", force_next_word, force_next_word_list)):
+            if flags is not None:
+                if flag:
+                    raise ValueError("pass either %s or %s_list, not both" % (name, name))
+                if len(flags) != n:
+                    raise ValueError("%s_list has %d entries for %d streams" % (name, len(flags), n))
         hot_list = weight_list = None
         if hotword_scorer_list is not None:
             if hotword_scorer is not None:
@@ -897,7 +916,13 @@ class BeamSearchDecoderCTC:
             starts.append(entry[2] if entry is not None else None)
         hot = hotword_scorer.unigrams if hotword_scorer is not None else None
         weight = hotword_scorer.weight if hotword_scorer is not None else DEFAULT_HOTWORD_WEIGHT
-        mode = _lib.FIN_EOS if is_end else (_lib.FIN_FLUSH if force_next_word else _lib.FIN_KEEP)
+        mode: Union[int, List[int]]
+        if is_end_list is None and force_next_word_list is None:
+            mode = _lib.FIN_EOS if is_end else (_lib.FIN_FLUSH if force_next_word else _lib.FIN_KEEP)
+        else:
+            ends = is_end_list if is_end_list is not None else [is_end] * n
+            forces = force_next_word_list if force_next_word_list is not None else [force_next_word] * n
+            mode = [_lib.FIN_EOS if e else (_lib.FIN_FLUSH if f else _lib.FIN_KEEP) for e, f in zip(ends, forces)]
         return self._run(logits_list, beam_width, beam_prune_logp, token_min_logp, prune_history, hot, weight,
                          max_out_beams=beam_width, lm_start_states=starts, with_state=False,
                          stream=[(list(b), int(p)) for b, p in zip(beams_list, processed_frames_list)], finalize_mode=mode,
