@@ -199,6 +199,17 @@ typedef struct {
      * B2C_FIN_KEEP], or finalize_mode != B2C_FIN_EOS together with utt_finalize_mode.  The call is a streaming call
      * when stream_states is given or some utterance's mode is not B2C_FIN_EOS. */
     const int32_t* utt_finalize_mode;
+    /* per-utterance search parameters: each NULL, or [n_utts] values; a given array replaces its scalar field
+     * (beam_width, beam_prune_logp, token_min_logp, prune_history) for every utterance, which is then decoded exactly
+     * as a call of its own with those values (batched streaming where streams run at different widths or thresholds),
+     * and returns at most min(max_out_beams, utt_beam_width[i]) beams.  Accepted only together with stream_states (they
+     * run on the general kernel), else B2C_E_ARG; B2C_E_ARG also for a width outside [1, 65535].  Both checks run
+     * before anything is enqueued.  The beam tables, candidate tiers, history-prune tables and arenas are sized by the
+     * call's largest width, and the shared-memory limit is checked against it. */
+    const int32_t* utt_beam_width;
+    const double* utt_beam_prune_logp;
+    const double* utt_token_min_logp;
+    const int32_t* utt_prune_history;
 } b2c_decode_opts_t;
 void b2c_decode_opts_default(b2c_decode_opts_t* opts);
 

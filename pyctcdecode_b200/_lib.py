@@ -64,6 +64,10 @@ class DecodeOpts(C.Structure):
         ("utt_lm_set", C.POINTER(C.c_int32)),
         ("lm_start_width", C.c_int),
         ("utt_finalize_mode", C.POINTER(C.c_int32)),
+        ("utt_beam_width", C.POINTER(C.c_int32)),
+        ("utt_beam_prune_logp", C.POINTER(C.c_double)),
+        ("utt_token_min_logp", C.POINTER(C.c_double)),
+        ("utt_prune_history", C.POINTER(C.c_int32)),
     ]
 
 

@@ -215,6 +215,9 @@ B2C_HD void b2c_beam_block(const B2cBeamArgs& A, int slot, u8* smem) {
         if (Tn > 0) rec = recs[0];
         B2cStreamIn sin{nullptr, 0u, nullptr, nullptr};
         int t0_frames = 0;
+        // the utterance's search parameters: a streaming call (general kernel only) carries them in its record, so
+        // that every reader below -- frame steps, in-place check, finalisation -- takes the utterance's own values
+        B2cParams P = A.P;
         if (A.s_utts) {
             const B2cStreamUtt su = A.s_utts[u];
             sin.beams = A.s_beams + su.beam_off;
@@ -222,8 +225,14 @@ B2C_HD void b2c_beam_block(const B2cBeamArgs& A, int slot, u8* smem) {
             sin.word_hash = A.s_word_hash;
             sin.word_len = A.s_word_len;
             t0_frames = su.t0;
+            if (!kFast) {
+                P.beam_width = su.beam_width;
+                P.prune_history = su.prune_history;
+                P.prune_logp = su.prune_logp;
+                P.bucket_scale = b2c_bucket_scale(su.prune_logp);
+            }
         }
-        b2c_utt_begin(A.P, W, u, A.start_states ? A.start_states + static_cast<u64>(u) * (A.P.lm_x + 1) : nullptr,
+        b2c_utt_begin(P, W, u, A.start_states ? A.start_states + static_cast<u64>(u) * (A.P.lm_x + 1) : nullptr,
                       static_cast<int>(rec.cnt), sin);
 #if defined(__CUDACC__)
 #pragma unroll 1
@@ -243,18 +252,18 @@ B2C_HD void b2c_beam_block(const B2cBeamArgs& A, int slot, u8* smem) {
                 single = t0.canon;
                 const int kind = b2c_inplace_kind(W.sc->flags, prev_single, t0.flags, t0.canon);
                 if (kind != B2C_INPLACE_NO)
-                    in_place = b2c_inplace_step(A.P, W, t + t0_frames, kind, id0, t0, rec.lp0, static_cast<int>(nxt.cnt));
+                    in_place = b2c_inplace_step(P, W, t + t0_frames, kind, id0, t0, rec.lp0, static_cast<int>(nxt.cnt));
                 B2C_MARK(5);
             }
             prev_single = single;
             if (in_place) {
                 // no table swap, no parity flip
             } else if (kFast && W.sc->n_beams * rec.cnt > L.cap_s) {
-                b2c_frame_step_slow(A.P, L, smem, g, parity, t + t0_frames, A.tok_ids + base, A.tok_lp + base, static_cast<int>(rec.cnt), static_cast<int>(nxt.cnt));
+                b2c_frame_step_slow(P, L, smem, g, parity, t + t0_frames, A.tok_ids + base, A.tok_lp + base, static_cast<int>(rec.cnt), static_cast<int>(nxt.cnt));
                 b2c_swap_tabs(W.cur, W.nxt);   // the out-of-line step swapped its private descriptor
                 parity ^= 1;
             } else {
-                b2c_frame_step<kFast>(A.P, W, t + t0_frames, A.tok_ids + base, A.tok_lp + base, static_cast<int>(rec.cnt), static_cast<int>(nxt.cnt));
+                b2c_frame_step<kFast>(P, W, t + t0_frames, A.tok_ids + base, A.tok_lp + base, static_cast<int>(rec.cnt), static_cast<int>(nxt.cnt));
                 parity ^= 1;
             }
             rec = nxt;
@@ -272,7 +281,7 @@ B2C_HD void b2c_beam_block(const B2cBeamArgs& A, int slot, u8* smem) {
         O.states = A.out_states + static_cast<u64>(u) * ob;
         O.aux = A.out_aux ? A.out_aux + 4 * static_cast<u64>(u) * ob : nullptr;
         O.states_x = A.out_states_x ? A.out_states_x + static_cast<u64>(u) * ob * A.P.lm_x : nullptr;
-        b2c_finalize(A.P, W, O, A.s_utts ? A.s_utts[u].fin_mode : A.fin_mode);
+        b2c_finalize(P, W, O, A.s_utts ? A.s_utts[u].fin_mode : A.fin_mode);
         B2C_MARK(8);
     }
     B2C_LEADER {
@@ -1469,6 +1478,28 @@ void b2c_decode_opts_default(b2c_decode_opts_t* o) {
 }
 
 // ---- decode call, stage by stage ----------------------------------------------------------------------------
+// the search parameters: the scalar fields, or one value per utterance (streaming calls only: they run on the general
+// kernel, which reads them from the utterance's B2cStreamUtt).  g.beam_width becomes the call's largest width, which
+// sizes the layout, the candidate tiers, the history-prune tables and the arenas.
+static int check_search_params(Call& c) {
+    const b2c_decode_opts_t* o = c.opts;
+    const bool per_utt = o->utt_beam_width || o->utt_beam_prune_logp || o->utt_token_min_logp || o->utt_prune_history;
+    if (per_utt && !o->stream_states) return fail(B2C_E_ARG, "per-utterance search parameters need stream_states");
+    if (!o->utt_beam_width) {
+        if (o->beam_width < 1) return fail(B2C_E_ARG, "beam_width must be >= 1");
+        if (o->beam_width > 65535) return fail(B2C_E_ARG, "beam_width above 65535 is not supported");
+        return 0;
+    }
+    int w_max = 1;
+    for (int i = 0; i < c.g.n_utts; ++i) {
+        const int w = o->utt_beam_width[i];
+        if (w < 1 || w > 65535) return fail(B2C_E_ARG, "utt_beam_width value outside [1, 65535]");
+        w_max = std::max(w_max, w);
+    }
+    c.g.beam_width = w_max;
+    return 0;
+}
+
 // batch geometry: frame offsets, longest-first order
 static int set_geometry(Call& c) {
     Geometry& g = c.g;
@@ -1484,13 +1515,13 @@ static int set_geometry(Call& c) {
     const int32_t* T = c.T;
     std::stable_sort(c.order.begin(), c.order.end(), [T](int a, int b) { return T[a] > T[b]; });
     g.order = c.order.data();
-    c.OB = std::max(1, std::min(c.opts->max_out_beams, c.opts->beam_width));
+    c.OB = std::max(1, std::min(c.opts->max_out_beams, g.beam_width));
     return 0;
 }
 
-// streaming input (partial_decode_beams): flatten the per-utterance beam / word lists and finalize modes.  Every
-// utterance of a streaming call gets a B2cStreamUtt record (zero input beams without stream_states): it carries the
-// utterance's finalize mode to the kernel.
+// streaming input (partial_decode_beams): flatten the per-utterance beam / word lists, finalize modes and search
+// parameters.  Every utterance of a streaming call gets a B2cStreamUtt record (zero input beams without stream_states):
+// it carries the utterance's finalize mode and search parameters to the kernel.
 static int flatten_stream_states(const b2c_decoder* d, Call& c) {
     const b2c_decode_opts_t* o = c.opts;
     Geometry& g = c.g;
@@ -1508,10 +1539,14 @@ static int flatten_stream_states(const b2c_decoder* d, Call& c) {
         c.s_utts.resize(g.n_utts);
         for (int i = 0; i < g.n_utts; ++i) {
             const int mode = modes ? modes[i] : o->finalize_mode;
-            if (!o->stream_states) { c.s_utts[i] = B2cStreamUtt{0u, 0u, 0, mode}; continue; }
+            const int width = o->utt_beam_width ? o->utt_beam_width[i] : o->beam_width;
+            const int prune_history = (o->utt_prune_history ? o->utt_prune_history[i] : o->prune_history) ? 1 : 0;
+            const double prune_logp = o->utt_beam_prune_logp ? o->utt_beam_prune_logp[i] : o->beam_prune_logp;
+            if (!o->stream_states) { c.s_utts[i] = B2cStreamUtt{0u, 0u, 0, mode, width, prune_history, prune_logp}; continue; }
             const b2c_stream_state_t& ss = o->stream_states[i];
             if (ss.n_beams < 0 || ss.n_beams > 65535 || (ss.n_beams > 0 && !ss.beams)) return fail(B2C_E_ARG, "bad stream state");
-            const B2cStreamUtt su{static_cast<u32>(c.s_beams.size()), static_cast<u32>(ss.n_beams), ss.processed_frames, mode};
+            const B2cStreamUtt su{static_cast<u32>(c.s_beams.size()), static_cast<u32>(ss.n_beams), ss.processed_frames, mode, width,
+                                  prune_history, prune_logp};
             const u32 wbase = static_cast<u32>(c.s_wh.size());
             u64 words = 0;
             for (int b = 0; b < ss.n_beams; ++b) {
@@ -1529,7 +1564,7 @@ static int flatten_stream_states(const b2c_decoder* d, Call& c) {
             g.s_max_words = std::max(g.s_max_words, words);
         }
     }
-    g.W_tab = std::max(o->beam_width, g.s_max_beams);     // capacity of the beam tables
+    g.W_tab = std::max(g.beam_width, g.s_max_beams);     // capacity of the beam tables
     return 0;
 }
 
@@ -1709,7 +1744,7 @@ static int make_params(b2c_decoder* d, Call& c) {
     const b2c_decode_opts_t* o = c.opts;
     B2cParams& P = c.P;
     P.V = c.g.V; P.is_bpe = d->is_bpe; P.has_dup_labels = d->has_dup_labels;
-    P.beam_width = o->beam_width; P.prune_history = o->prune_history ? 1 : 0; P.out_beams = c.OB; P.narrow_chain = c.text_only ? 1 : 0;
+    P.beam_width = c.g.beam_width; P.prune_history = o->prune_history ? 1 : 0; P.out_beams = c.OB; P.narrow_chain = c.text_only ? 1 : 0;
     P.prune_logp = o->beam_prune_logp; P.token_min_logp = o->token_min_logp;
     P.bucket_scale = b2c_bucket_scale(o->beam_prune_logp);
     P.kflags = c.k.no_single ? B2C_FL_NO_SINGLE : 0;
@@ -1849,8 +1884,9 @@ static int upload(b2c_decoder* d, Call& c) {
     }
     if (!c.s_utts.empty()) {
         const size_t b0 = al16(sizeof(B2cStreamUtt) * c.s_utts.size()), b1 = al16(sizeof(B2cStreamBeam) * std::max<size_t>(c.s_beams.size(), 1)),
-                     b2 = al16(8 * std::max<size_t>(c.s_wh.size(), 1)), b3 = al16(4 * std::max<size_t>(c.s_wl.size(), 1));
-        if (d->d_stream.ensure(b0 + b1 + b2 + b3)) return B2C_E_NOMEM;
+                     b2 = al16(8 * std::max<size_t>(c.s_wh.size(), 1)), b3 = al16(4 * std::max<size_t>(c.s_wl.size(), 1)),
+                     b4 = c.opts->utt_token_min_logp ? al16(8ull * n) : 0;
+        if (d->d_stream.ensure(b0 + b1 + b2 + b3 + b4)) return B2C_E_NOMEM;
         u8* base = d->d_stream.as<u8>();
         CUDA_OK(cudaMemcpyAsync(base, c.s_utts.data(), sizeof(B2cStreamUtt) * c.s_utts.size(), cudaMemcpyHostToDevice, st));
         if (!c.s_beams.empty()) CUDA_OK(cudaMemcpyAsync(base + b0, c.s_beams.data(), sizeof(B2cStreamBeam) * c.s_beams.size(), cudaMemcpyHostToDevice, st));
@@ -1860,7 +1896,11 @@ static int upload(b2c_decoder* d, Call& c) {
         }
         c.BA.s_utts = reinterpret_cast<const B2cStreamUtt*>(base); c.BA.s_beams = reinterpret_cast<const B2cStreamBeam*>(base + b0);
         c.BA.s_word_hash = reinterpret_cast<const u64*>(base + b0 + b1); c.BA.s_word_len = reinterpret_cast<const u32*>(base + b0 + b1 + b2);
-        d->tm.h2d_bytes += static_cast<long long>(b0 + b1 + b2 + b3);
+        if (b4) {      // the streaming stage's per-utterance token thresholds
+            CUDA_OK(cudaMemcpyAsync(base + b0 + b1 + b2 + b3, c.opts->utt_token_min_logp, 8ull * n, cudaMemcpyHostToDevice, st));
+            c.PA.utt_token_min_logp = reinterpret_cast<const double*>(base + b0 + b1 + b2 + b3);
+        }
+        d->tm.h2d_bytes += static_cast<long long>(b0 + b1 + b2 + b3 + b4);
     }
     return 0;
 }
@@ -2110,7 +2150,7 @@ static int read_back(b2c_decoder* d, Call& c) {
     d->tm.d2h_bytes += static_cast<long long>(c.out.bytes + c.tok_bytes + (c.text_only ? 0 : c.frm_bytes) + 8ull * n + 32);
     const u32* ms = d->h_mstats.as<u32>();
     d->hint_valid = true;
-    d->hint_beam = c.opts->beam_width; d->hint_lm = c.any_lm ? 1 : 0; d->hint_hot = c.any_hot ? 1 : 0; d->hint_prune = c.P.prune_history;
+    d->hint_beam = c.g.beam_width; d->hint_lm = c.any_lm ? 1 : 0; d->hint_hot = c.any_hot ? 1 : 0; d->hint_prune = c.P.prune_history;
     for (int q = 0; q < 6; ++q) d->hint_over[q] = ms[q];
     d->hint_frames = ms[6];
     for (int q = 0; q < 7; ++q) d->tm.cand_hist[q] = ms[q];
@@ -2265,8 +2305,7 @@ static int decode_batch_locked(b2c_decoder_t* d, const void* const* logits, cons
     if (dtype < B2C_DTYPE_F32 || dtype > B2C_DTYPE_BF16) return fail(B2C_E_ARG, "dtype must be one of B2C_DTYPE_F32 / F64 / F16 / BF16");
     Call c(d, logits, T, n_utts, dtype, is_device, opts, allow_pipe);
     d->last_T.clear();
-    if (opts->beam_width < 1) return fail(B2C_E_ARG, "beam_width must be >= 1");
-    if (opts->beam_width > 65535) return fail(B2C_E_ARG, "beam_width above 65535 is not supported");
+    B2C_TRY(check_search_params(c));
     std::unique_ptr<b2c_result> res(new b2c_result());
     res->utts.resize(n_utts); res->has_lm = d->lm != nullptr;
     if (n_utts == 0) { *out = res.release(); return 0; }

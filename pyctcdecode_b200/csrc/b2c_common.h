@@ -263,7 +263,9 @@ struct B2cStreamBeam {
     u32 last_tok;              // canonical token id of last_char, B2C_NO_TOK for None
     int pf_s, pf_e;            // partial_frames
 };
-struct B2cStreamUtt { u32 beam_off, n_beams; int t0; int fin_mode; };   // t0: processed_frames; fin_mode: B2C_FIN_*
+// t0: processed_frames; fin_mode: B2C_FIN_*; beam_width / prune_history / prune_logp: the utterance's search parameters
+// (the call's values unless the call gives them per utterance), read in place of B2cParams' by the general kernel
+struct B2cStreamUtt { u32 beam_off, n_beams; int t0; int fin_mode; int beam_width, prune_history; double prune_logp; };
 // what _finalize_beams does at the end of a call (decoder.py:558-602); same values as include/b200ctc.h
 #ifndef B2C_FIN_EOS
 #define B2C_FIN_EOS 0          // force_next_word or is_end, scored with is_eos=True (decode_beams; is_end=True)

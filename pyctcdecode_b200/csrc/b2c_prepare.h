@@ -267,6 +267,7 @@ struct B2cPrepArgs {
     u64 total_frames;
     int V;
     double token_min_logp;
+    const double* utt_token_min_logp;  // [B] per-utterance thresholds (streaming calls that give them), or NULL: token_min_logp
     B2cFrameRec* tok_rec;    // [total_frames]
     u32* tok_ids;            // [total_frames * V]  (32-bit: the beam kernel stages them with 4-byte cp.async)
     double* tok_lp;
@@ -284,6 +285,9 @@ struct B2cPrepArgs {
     u32* max_k;              // [B] largest per-frame token count (zeroed before the launch)
     u32* sum_k;              // [B] total number of selected tokens (zeroed before the launch)
 };
+
+// the token threshold of utterance u
+B2C_HD double b2c_token_min_of(const B2cPrepArgs& A, int u) { return A.utt_token_min_logp ? A.utt_token_min_logp[u] : A.token_min_logp; }
 
 // ---- rowsum ---------------------------------------------------------------------------------
 template <class T>
@@ -714,6 +718,7 @@ B2C_HD void b2c_tokens_run_v32(const B2cPrepArgs& A, u64 run, int lane, u16* set
     const u64 f0 = A.frame_off[u];
     if (A.mode == 1 && A.is_prob[u] == 0) return;          // second pass: probability utterances only
     const bool is_prob = A.mode == 1;
+    const double thr = b2c_token_min_of(A, u);
     const T* x = static_cast<const T*>(A.logits) + f0 * static_cast<u64>(V);
     const u64 base = (f0 + static_cast<u64>(t0)) * static_cast<u64>(V);
     if (A.mode == 0) b2c_accum_approx<T>(A.approx + 2 * u, x + static_cast<u64>(t0) * V, static_cast<long>(nf) * V, lane);
@@ -733,7 +738,7 @@ B2C_HD void b2c_tokens_run_v32(const B2cPrepArgs& A, u64 run, int lane, u16* set
             double ls;
             int amax;
             u32 mask;
-            b2c_prep_row<T, true>(x + static_cast<u64>(t0 + f) * V, V, is_prob, A.token_min_logp, lane, set, m, ls, amax, mask);
+            b2c_prep_row<T, true>(x + static_cast<u64>(t0 + f) * V, V, is_prob, thr, lane, set, m, ls, amax, mask);
             amax = __shfl_sync(full, amax, 0);          // lane 0's view, like the general path
             if (lane == f) { my_mask = mask; my_amax = static_cast<u32>(amax); my_m = m; my_ls = ls; }
         }
@@ -776,7 +781,7 @@ B2C_HD void b2c_tokens_run_v32(const B2cPrepArgs& A, u64 run, int lane, u16* set
         double ls;
         int amax;
         u32 ns;
-        b2c_prep_row<T, false>(row, V, is_prob, A.token_min_logp, lane, set, m, ls, amax, ns);
+        b2c_prep_row<T, false>(row, V, is_prob, thr, lane, set, m, ls, amax, ns);
         u32 off = __shfl_sync(full, my_off, f);
         if (lane == 0) {
             b2c_pyset_copy_or(set, static_cast<u32>(amax));
@@ -818,7 +823,7 @@ B2C_HD void b2c_tokens_run_v32(const B2cPrepArgs& A, u64 run, int lane, u16* set
         double ls;
         int amax;
         u32 mask;
-        b2c_prep_row<T, true>(row, V, is_prob, A.token_min_logp, 0, set, m, ls, amax, mask);
+        b2c_prep_row<T, true>(row, V, is_prob, thr, 0, set, m, ls, amax, mask);
         u32 nsel = 0;
         for (u32 b = 0; b < 32; ++b) nsel += (mask >> b) & 1u;
         const bool small = nsel == 0 || (nsel <= 3 && ((mask >> amax) & 1u));
@@ -838,7 +843,7 @@ B2C_HD void b2c_tokens_run_v32(const B2cPrepArgs& A, u64 run, int lane, u16* set
             rec.cnt = static_cast<u16>(n);
         } else {
             u32 ns;
-            b2c_prep_row<T, false>(row, V, is_prob, A.token_min_logp, 0, set, m, ls, amax, ns);
+            b2c_prep_row<T, false>(row, V, is_prob, thr, 0, set, m, ls, amax, ns);
             b2c_pyset_copy_or(set, static_cast<u32>(amax));
             rec.cnt = static_cast<u16>(set.fill);
             const u16* tab = set.buf[set.cur];
@@ -876,6 +881,7 @@ B2C_HD void b2c_tokens_run(const B2cPrepArgs& A, u64 run, int lane, u16* set0, u
     const u64 f0 = A.frame_off[u];
     if (A.mode == 1 && A.is_prob[u] == 0) return;          // second pass: probability utterances only
     const bool is_prob = A.mode == 1;
+    const double thr = b2c_token_min_of(A, u);
     const T* x = static_cast<const T*>(A.logits) + f0 * static_cast<u64>(V);
     const u64 base = (f0 + static_cast<u64>(t0)) * static_cast<u64>(V);
 #if defined(__CUDA_ARCH__)
@@ -907,15 +913,15 @@ B2C_HD void b2c_tokens_run(const B2cPrepArgs& A, u64 run, int lane, u16* set0, u
                 float fm, fsx, fsa;
                 const float* const frow = reinterpret_cast<const float*>(row);
                 const bool vec4 = (V & 3) == 0 && (reinterpret_cast<unsigned long long>(frow) & 15ull) == 0;
-                row_done = vec4 ? b2c_prep_row_f32_fast4(frow, V, A.token_min_logp, lane, set, fm, ls, amax, nsel, fsx, fsa)
-                                : b2c_prep_row_f32_fast(frow, V, A.token_min_logp, lane, set, fm, ls, amax, nsel, fsx, fsa);
+                row_done = vec4 ? b2c_prep_row_f32_fast4(frow, V, thr, lane, set, fm, ls, amax, nsel, fsx, fsa)
+                                : b2c_prep_row_f32_fast(frow, V, thr, lane, set, fm, ls, amax, nsel, fsx, fsa);
                 m = fm;
                 run_sx += static_cast<double>(fsx);
                 run_sa += static_cast<double>(fsa);
             }
         }
 #endif
-        if (!row_done) b2c_prep_row<T, false>(row, V, is_prob, A.token_min_logp, lane, set, m, ls, amax, nsel);
+        if (!row_done) b2c_prep_row<T, false>(row, V, is_prob, thr, lane, set, m, ls, amax, nsel);
         if (lane == 0) {
             b2c_pyset_copy_or(set, static_cast<u32>(amax));
             const u32 cnt = set.fill;
@@ -1065,7 +1071,6 @@ __device__ inline void b2c_tokens_tiles_v32(const B2cPrepArgs& A, int block_idx,
     B2cTileInfo cur = b2c_tile_locate(A, gw);
     b2c_tile_issue(cur, sh->tile[w][0], &sh->mbar[w][0], lane);
     const int lr = lane % V;                 // rotation of this lane's walk over its row
-    const double thr = A.token_min_logp;
     for (u64 tile = gw; tile < total; tile += n_warps) {
         B2cTileInfo nxt;
         nxt.nrows = 0;
@@ -1088,6 +1093,7 @@ __device__ inline void b2c_tokens_tiles_v32(const B2cPrepArgs& A, int block_idx,
             for (int i = lane; i < n; i += 32) T0[i] = cur.src[i];
             __syncwarp();
         }
+        const double thr = b2c_token_min_of(A, cur.u);      // every row of a tile belongs to one utterance
         // ---- one row per lane ----------------------------------------------------------------------------------
         const bool mine = lane < cur.nrows;
         const float* row = T0 + lane * V;

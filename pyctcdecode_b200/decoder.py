@@ -328,7 +328,8 @@ class BeamSearchDecoderCTC:
              stream: Optional[Sequence[Tuple[Sequence[Beam], int]]] = None, finalize_mode: Union[int, List[int]] = _lib.FIN_EOS,
              hotwords_list: Optional[Sequence[Optional[Iterable[str]]]] = None,
              hotword_weight_list: Optional[Sequence[float]] = None,
-             language_model_list: Optional[Sequence[Optional[AbstractLanguageModel]]] = None) -> Any:
+             language_model_list: Optional[Sequence[Optional[AbstractLanguageModel]]] = None,
+             utt_search: Optional[Dict[str, List[Any]]] = None) -> Any:
         packed = self._as_packed_batch(logits_list)
         if lengths is not None and packed is None:
             raise ValueError("lengths= needs one padded [B, T, V] array or tensor")
@@ -380,7 +381,7 @@ class BeamSearchDecoderCTC:
         with self._run_lock:
             return self._run_locked(mats, n, dtype_code, is_device, device, torch_stream, beam_width, beam_prune_logp,
                                     token_min_logp, prune_history, hotwords, hotword_weight, max_out_beams, lm_start_states,
-                                    with_state, texts_only, stream, finalize_mode, utt_hot, utt_lms)
+                                    with_state, texts_only, stream, finalize_mode, utt_hot, utt_lms, utt_search)
 
     def _run_locked(self, mats: List[Tuple[Any, int, int, int, bool]], n: int, dtype_code: int, is_device: bool,
                     device: Optional[int], torch_stream: Optional[int], beam_width: int, beam_prune_logp: float,
@@ -388,7 +389,8 @@ class BeamSearchDecoderCTC:
                     max_out_beams: int, lm_start_states: Optional[Sequence[Optional[AbstractLMState]]], with_state: bool,
                     texts_only: bool, stream: Optional[Sequence[Tuple[Sequence[Beam], int]]], finalize_mode: Union[int, List[int]],
                     utt_hot: Optional[List[Tuple[List[str], float]]] = None,
-                    utt_lms: Optional[List[List[LanguageModel]]] = None) -> Any:
+                    utt_lms: Optional[List[List[LanguageModel]]] = None,
+                    utt_search: Optional[Dict[str, List[Any]]] = None) -> Any:
         handle = self._handle(device)
         L = _lib.lib()
         if torch_stream is not None:
@@ -410,6 +412,12 @@ class BeamSearchDecoderCTC:
         opts.n_hotwords = len(hot)
         opts.hotword_weight = float(hotword_weight)
         keep_alive: List[Any] = []
+        for field, ctype in (("beam_width", C.c_int32), ("beam_prune_logp", C.c_double), ("token_min_logp", C.c_double),
+                             ("prune_history", C.c_int32)):
+            if utt_search is not None and field in utt_search:      # one value per stream (streaming calls only)
+                arr = (ctype * n)(*utt_search[field])
+                keep_alive.append(arr)
+                setattr(opts, "utt_" + field, C.cast(arr, C.POINTER(ctype)))
         if utt_hot is not None:
             # utterances with the same (hotwords, weight) share one set; the weight is compared bit for bit
             set_of: Dict[Tuple[Tuple[str, ...], bytes], int] = {}
@@ -877,7 +885,11 @@ class BeamSearchDecoderCTC:
                                    hotword_scorer_list: Optional[Sequence[Optional[HotwordScorer]]] = None,
                                    language_model_list: Optional[Sequence[Optional[AbstractLanguageModel]]] = None,
                                    is_end_list: Optional[Sequence[bool]] = None,
-                                   force_next_word_list: Optional[Sequence[bool]] = None) -> List[List[LMBeam]]:
+                                   force_next_word_list: Optional[Sequence[bool]] = None,
+                                   beam_width_list: Optional[Sequence[Optional[int]]] = None,
+                                   beam_prune_logp_list: Optional[Sequence[Optional[float]]] = None,
+                                   token_min_logp_list: Optional[Sequence[Optional[float]]] = None,
+                                   prune_history_list: Optional[Sequence[Optional[bool]]] = None) -> List[List[LMBeam]]:
         """Extension: many independent streams advance by one chunk each in ONE kernel launch.  `hotword_scorer_list`:
         one HotwordScorer (or None) per stream instead of one `hotword_scorer` for all.
 
@@ -891,7 +903,13 @@ class BeamSearchDecoderCTC:
         `is_end_list` / `force_next_word_list`: one flag per stream instead of `is_end` / `force_next_word` for all, so
         that streams that end, streams that flush their partial word and streams that go on share one call.  Stream i
         then gets what ``partial_decode_beams(..., force_next_word=force_next_word_list[i], is_end=is_end_list[i])``
-        returns for it."""
+        returns for it.
+
+        `beam_width_list` / `beam_prune_logp_list` / `token_min_logp_list` / `prune_history_list`: one value per stream
+        instead of `beam_width` / `beam_prune_logp` / `token_min_logp` / `prune_history` for all (an entry of None takes
+        the scalar), so that streams with different accuracy and latency settings share one call.  Stream i then gets
+        what ``partial_decode_beams(..., beam_width=w_i, beam_prune_logp=p_i, token_min_logp=t_i, prune_history=h_i)``
+        returns for it.  The call is laid out for its largest width."""
         n = len(logits_list)
         if not (len(beams_list) == len(processed_frames_list) == len(cached_lm_scores_list) == n):
             raise ValueError("one beam list, cache and processed_frames value per stream")
@@ -901,6 +919,23 @@ class BeamSearchDecoderCTC:
                     raise ValueError("pass either %s or %s_list, not both" % (name, name))
                 if len(flags) != n:
                     raise ValueError("%s_list has %d entries for %d streams" % (name, len(flags), n))
+        utt_search: Optional[Dict[str, List[Any]]] = None
+        widths = [beam_width] * n
+        for name, scalar, values, conv in (("beam_width", beam_width, beam_width_list, int),
+                                           ("beam_prune_logp", beam_prune_logp, beam_prune_logp_list, float),
+                                           ("token_min_logp", token_min_logp, token_min_logp_list, float),
+                                           ("prune_history", prune_history, prune_history_list, lambda h: int(bool(h)))):
+            if values is None:
+                continue
+            if len(values) != n:
+                raise ValueError("%s_list has %d entries for %d streams" % (name, len(values), n))
+            resolved = [conv(scalar if v is None else v) for v in values]
+            if name == "beam_width":
+                if any(w < 1 or w > 65535 for w in resolved):
+                    raise ValueError("beam_width_list entries must lie in [1, 65535]")
+                widths = resolved
+            utt_search = utt_search if utt_search is not None else {}
+            utt_search[name] = resolved
         hot_list = weight_list = None
         if hotword_scorer_list is not None:
             if hotword_scorer is not None:
@@ -924,9 +959,10 @@ class BeamSearchDecoderCTC:
             forces = force_next_word_list if force_next_word_list is not None else [force_next_word] * n
             mode = [_lib.FIN_EOS if e else (_lib.FIN_FLUSH if f else _lib.FIN_KEEP) for e, f in zip(ends, forces)]
         return self._run(logits_list, beam_width, beam_prune_logp, token_min_logp, prune_history, hot, weight,
-                         max_out_beams=beam_width, lm_start_states=starts, with_state=False,
-                         stream=[(list(b), int(p)) for b, p in zip(beams_list, processed_frames_list)], finalize_mode=mode,
-                         hotwords_list=hot_list, hotword_weight_list=weight_list, language_model_list=language_model_list)
+                         max_out_beams=max(widths) if utt_search is not None and n else beam_width, lm_start_states=starts,
+                         with_state=False, stream=[(list(b), int(p)) for b, p in zip(beams_list, processed_frames_list)],
+                         finalize_mode=mode, hotwords_list=hot_list, hotword_weight_list=weight_list,
+                         language_model_list=language_model_list, utt_search=utt_search)
 
     # ---- serialisation (reference decoder.py:947-1005): file plumbing only ------------------
     def save_to_dir(self, filepath: str) -> None:
