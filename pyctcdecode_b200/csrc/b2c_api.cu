@@ -160,7 +160,8 @@ struct B2cBeamArgs {
     double* out_scores;
     int* out_ntok;
     int* out_nwords;
-    u32* out_toks;
+    u32* out_toks;             // text-only calls: the transcripts' byte regions, (u, r) at ((f0 + u) * out_beams + r * (T + 1))
+                               // * P.text_node_bytes (B2cOut::text); no token chains, no word frames
     int* out_frames;
     B2cLmState* out_states;
     // chunked launches of the latency-first kernel (chunk_t1 > 0): frames [chunk_t0, chunk_t1) of every utterance, CTA i
@@ -281,6 +282,7 @@ B2C_HD void b2c_beam_block(const B2cBeamArgs& A, int slot, u8* smem) {
         O.states = A.out_states + static_cast<u64>(u) * ob;
         O.aux = A.out_aux ? A.out_aux + 4 * static_cast<u64>(u) * ob : nullptr;
         O.states_x = A.out_states_x ? A.out_states_x + static_cast<u64>(u) * ob * A.P.lm_x : nullptr;
+        O.text = reinterpret_cast<u8*>(A.out_toks) + ob * (f0 + static_cast<u64>(u)) * A.P.text_node_bytes;
         b2c_finalize(P, W, O, A.s_utts ? A.s_utts[u].fin_mode : A.fin_mode);
         B2C_MARK(8);
     }
@@ -338,6 +340,68 @@ B2C_HD void b2c_widen_range(const u16* src, float* dst, u64 begin, u64 end, u64 
     for (u64 i = begin; i < end; i += step) dst[i] = bf16 ? b2c_bf16_bits_to_float(src[i]) : b2c_f16_bits_to_float(src[i]);
 }
 
+// Text-only calls: the transcripts of every output beam, back to back, each followed by '\0' (an utterance without an
+// output beam has one empty entry), behind a u64 header that holds their total size.  Slot s = u * out_beams + r; CTA b
+// joins the slots [b, b + 1) * B2C_JOIN_TILE after summing the sizes of the slots in front of them.
+#define B2C_JOIN_TILE 32
+#define B2C_JOIN_THREADS 256
+struct B2cJoinArgs {
+    int n_utts, out_beams;
+    u32 node_bytes, pad;
+    const int* n_beams;
+    const int* len;            // B2cOut::n_tok
+    const u64* frame_off;
+    const int* T;
+    const u8* text;            // B2cBeamArgs::out_toks of a text-only call
+    u8* joined;
+};
+struct B2cJoinShared { u64 base; u32 off[B2C_JOIN_TILE + 1]; };
+// the end of slot s's region of `text` (its transcript is the last len bytes)
+B2C_HD const u8* b2c_join_end(const B2cJoinArgs& J, int s) {
+    const int u = s / J.out_beams, r = s % J.out_beams;
+    const u64 nodes = static_cast<u64>(J.T[u]) + 1;
+    return J.text + (static_cast<u64>(J.out_beams) * (J.frame_off[u] + static_cast<u64>(u)) + (static_cast<u64>(r) + 1) * nodes) * J.node_bytes;
+}
+// bytes of slot s in the joined buffer; a length is clamped to its region, so that an utterance that has to be decoded
+// again (whose first pass may have left anything) reads inside it
+B2C_HD u32 b2c_join_size(const B2cJoinArgs& J, int s) {
+    const int u = s / J.out_beams, r = s % J.out_beams;
+    if (r >= J.n_beams[u]) return r == 0 ? 1u : 0u;
+    const u32 cap = static_cast<u32>(J.T[u] + 1) * J.node_bytes, len = static_cast<u32>(J.len[s]);
+    return (len < cap ? len : cap) + 1u;
+}
+B2C_HD void b2c_join_block(const B2cJoinArgs& J, int b, B2cJoinShared* sh) {
+    const int S = J.n_utts * J.out_beams, s0 = b * B2C_JOIN_TILE;
+    const int n = S - s0 < B2C_JOIN_TILE ? S - s0 : B2C_JOIN_TILE;
+    B2C_LEADER { sh->base = 0; }
+    B2C_SYNC();
+    u64 part = 0;
+    B2C_FOR(s, s0) { part += b2c_join_size(J, s); }
+#if defined(__CUDA_ARCH__)
+    atomicAdd(reinterpret_cast<unsigned long long*>(&sh->base), static_cast<unsigned long long>(part));
+#else
+    sh->base += part;
+#endif
+    B2C_SYNC();
+    B2C_LEADER {
+        u32 o = 0;
+        for (int k = 0; k < n; ++k) { sh->off[k] = o; o += b2c_join_size(J, s0 + k); }
+        sh->off[n] = o;
+        if (s0 + n == S) *reinterpret_cast<u64*>(J.joined) = sh->base + o;
+    }
+    B2C_SYNC();
+    u8* out = J.joined + 8 + sh->base;
+    B2C_FOR(i, sh->off[n]) {
+        int lo = 0, hi = n;      // the slot k with off[k] <= i < off[k + 1]
+        while (hi - lo > 1) {
+            const int mid = (lo + hi) >> 1;
+            if (sh->off[mid] <= static_cast<u32>(i)) lo = mid; else hi = mid;
+        }
+        const u32 j = static_cast<u32>(i) - sh->off[lo], size = sh->off[lo + 1] - sh->off[lo];
+        out[i] = j + 1 < size ? (b2c_join_end(J, s0 + lo) - (size - 1))[j] : static_cast<u8>(0);
+    }
+}
+
 #ifndef B2C_HOSTSIM
 __global__ void __launch_bounds__(256) b2c_widen_kernel(const u16* src, float* dst, u64 n, int bf16) {
     b2c_widen_range(src, dst, static_cast<u64>(blockIdx.x) * blockDim.x + threadIdx.x, n, static_cast<u64>(gridDim.x) * blockDim.x, bf16);
@@ -372,6 +436,10 @@ template <class T>
 __global__ void __launch_bounds__(B2C_PREP_THREADS, 4) b2c_tokens_kernel(const B2cPrepArgs A) {
     __shared__ B2cPrepShared sh;
     b2c_tokens_block<T>(A, static_cast<int>(blockIdx.x), static_cast<int>(gridDim.x), &sh);
+}
+__global__ void __launch_bounds__(B2C_JOIN_THREADS) b2c_join_kernel(const B2cJoinArgs J) {
+    __shared__ B2cJoinShared sh;
+    b2c_join_block(J, static_cast<int>(blockIdx.x), &sh);
 }
 // kThreads x kOcc bound the register allocation: (128,4) and (256,2) -> <= 128 registers, (128,2) -> <= 255
 template <bool kFast, int kThreads, int kOcc>
@@ -550,6 +618,32 @@ struct b2c_decoder {
     int hint_beam = 0, hint_lm = 0, hint_hot = 0, hint_prune = 0;
     u32 hint_over[6] = {0, 0, 0, 0, 0, 0};
     u32 hint_frames = 0;
+    // text-only calls: the most bytes one backtrack node adds to a transcript (B2cParams::text_node_bytes), the
+    // transcripts' regions and their joined copy
+    DevBuf d_text, d_join;
+    PinBuf h_join;
+    u32 node_bytes = 1;
+};
+
+// the small-output block (device, then pinned host copy)
+struct OutViews {
+    int *nbeams, *status; double* scores; int *ntok, *nwords; B2cLmState* states;
+    int* aux;                     // streaming calls only
+    B2cLmState* states_x;         // MultiLanguageModel only
+};
+struct OutLayout {
+    u64 st = 0, sc = 0, nt = 0, nw = 0, ls = 0, ax = 0, lx = 0, bytes = 0;   // n_beams at 0
+    bool has_aux = false, has_x = false;
+    OutLayout() = default;
+    OutLayout(int n, int OB, int n_lm, bool streaming)
+        : st(al16(4ull * n)), sc(st + al16(4ull * n)), nt(sc + al16(16ull * OB * n)), nw(nt + al16(4ull * OB * n)), ls(nw + al16(4ull * OB * n)),
+          ax(ls + al16(sizeof(B2cLmState) * static_cast<u64>(OB) * n)), lx(ax + (streaming ? al16(16ull * OB * n) : 0)),
+          bytes(lx + al16(sizeof(B2cLmState) * static_cast<u64>(OB) * n * static_cast<u64>(n_lm - 1))), has_aux(streaming), has_x(n_lm > 1) {}
+    OutViews at(u8* b) const {
+        return OutViews{reinterpret_cast<int*>(b), reinterpret_cast<int*>(b + st), reinterpret_cast<double*>(b + sc),
+                        reinterpret_cast<int*>(b + nt), reinterpret_cast<int*>(b + nw), reinterpret_cast<B2cLmState*>(b + ls),
+                        has_aux ? reinterpret_cast<int*>(b + ax) : nullptr, has_x ? reinterpret_cast<B2cLmState*>(b + lx) : nullptr};
+    }
 };
 
 struct BeamRes {
@@ -565,7 +659,15 @@ struct BeamRes {
     int aux[4] = {-1, -1, -1, -1};
 };
 struct b2c_result {
-    std::vector<std::vector<BeamRes>> utts;
+    mutable std::vector<std::vector<BeamRes>> utts;   // text-only results: filled on first use (beams_of)
+    // text-only calls: the transcripts as the device joined them (b2c_join_block) and a copy of the small outputs; the
+    // beams are built from them only when something other than b2c_result_top_texts asks
+    bool text_only = false;
+    int OB = 1;
+    std::string texts;
+    std::vector<u8> small;
+    OutLayout out;
+    mutable std::once_flag built;
     bool has_lm = false;       // some utterance has a language model
     std::vector<int> utt_models;  // [n_utts] models of each utterance's set (0: none)
     std::string joined;        // b2c_result_top_texts: top-1 texts, each followed by '\0'
@@ -629,28 +731,6 @@ static u32 build_hot(const char* const* words, int n_words, std::vector<B2cHot>&
     return min_len_all;
 }
 
-// decode() / decode_batch() want the text only: no word vector, no frames
-static void assemble_text(const b2c_decoder* d, const u32* toks, int nt, BeamRes& br) {
-    br.text.clear();
-    br.text.reserve(static_cast<size_t>(nt > 0 ? nt : 0) + 16);      // one allocation (most tokens are one byte)
-    br.words.clear();
-    br.frames.clear();
-    bool open_word = false;      // the current word has at least one character
-    bool need_space = false;     // a finished word precedes
-    for (int i = nt - 1; i >= 0; --i) {
-        const u32 tok = toks[i] & 0xFFFFu, kind = toks[i] >> 16;
-        if (kind != B2C_CK_CONT) {       // word boundary: space, or a BPE piece that starts the next word
-            if (open_word) need_space = true;
-            open_word = false;
-            if (kind != B2C_CK_BPE) continue;
-        }
-        const std::string& piece = kind == B2C_CK_CONT ? d->labels[tok] : d->clean[tok];
-        if (piece.empty()) continue;
-        if (!open_word && need_space) br.text += ' ';
-        br.text += piece;
-        open_word = true;
-    }
-}
 static void assemble_beam(const b2c_decoder* d, const u32* toks, int nt, const int* frames, int nw, BeamRes& br) {
     std::string word;
     br.words.clear();
@@ -832,27 +912,6 @@ struct MetaLayout {
         : T(al16(8ull * n)), run(T + al16(4ull * n)), ord(run + al16(8ull * (n + 1))), next(ord + 2 * al16(4ull * n)), ptr(next + 64),
           bytes(ptr + al16(8ull * n)) {}
 };
-// the small-output block (device, then pinned host copy)
-struct OutViews {
-    int *nbeams, *status; double* scores; int *ntok, *nwords; B2cLmState* states;
-    int* aux;                     // streaming calls only
-    B2cLmState* states_x;         // MultiLanguageModel only
-};
-struct OutLayout {
-    u64 st = 0, sc = 0, nt = 0, nw = 0, ls = 0, ax = 0, lx = 0, bytes = 0;   // n_beams at 0
-    bool has_aux = false, has_x = false;
-    OutLayout() = default;
-    OutLayout(int n, int OB, int n_lm, bool streaming)
-        : st(al16(4ull * n)), sc(st + al16(4ull * n)), nt(sc + al16(16ull * OB * n)), nw(nt + al16(4ull * OB * n)), ls(nw + al16(4ull * OB * n)),
-          ax(ls + al16(sizeof(B2cLmState) * static_cast<u64>(OB) * n)), lx(ax + (streaming ? al16(16ull * OB * n) : 0)),
-          bytes(lx + al16(sizeof(B2cLmState) * static_cast<u64>(OB) * n * static_cast<u64>(n_lm - 1))), has_aux(streaming), has_x(n_lm > 1) {}
-    OutViews at(u8* b) const {
-        return OutViews{reinterpret_cast<int*>(b), reinterpret_cast<int*>(b + st), reinterpret_cast<double*>(b + sc),
-                        reinterpret_cast<int*>(b + nt), reinterpret_cast<int*>(b + nw), reinterpret_cast<B2cLmState*>(b + ls),
-                        has_aux ? reinterpret_cast<int*>(b + ax) : nullptr, has_x ? reinterpret_cast<B2cLmState*>(b + lx) : nullptr};
-    }
-};
-
 // opt-in host-side section timing (B200CTC_HOST_PROFILE=1, stderr)
 struct HostProfile {
     std::chrono::steady_clock::time_point t0 = std::chrono::steady_clock::now();
@@ -885,6 +944,7 @@ struct Call {
     MetaLayout meta;
     OutLayout out;
     u64 tok_bytes = 0, frm_bytes = 0;
+    u64 join_bytes = 0, join_first = 0;   // text-only calls: bound of the joined transcripts, bytes of them read back at once
     u32 set_cap = 16;
     int runs_per_utt = 1, tiles_per_utt = 1;
     u8 *hm = nullptr, *dm = nullptr;   // metadata block: host, device
@@ -1406,8 +1466,21 @@ int b2c_decoder_create(const char* const* labels, int n_labels, int is_bpe, b2c_
     d->n_sm = v;
     CUDA_OK(cudaDeviceGetAttribute(&v, cudaDevAttrMaxSharedMemoryPerBlockOptin, device));
     d->smem_optin = static_cast<size_t>(v);
-    if (d->d_toks.ensure(sizeof(B2cTok) * n_labels)) return B2C_E_NOMEM;
-    CUDA_OK(cudaMemcpy(d->d_toks.p, d->toks.data(), sizeof(B2cTok) * n_labels, cudaMemcpyHostToDevice));
+    std::vector<u8> pieces(sizeof(B2cPiece) * 2 * n_labels);
+    u32 longest = 0;
+    for (int i = 0; i < 2 * n_labels; ++i) {
+        const std::string& s = (i & 1) ? d->clean[i / 2] : d->labels[i / 2];
+        const B2cPiece pc{static_cast<u32>(pieces.size()), static_cast<u32>(s.size())};
+        std::memcpy(pieces.data() + sizeof(B2cPiece) * i, &pc, sizeof(pc));
+        pieces.insert(pieces.end(), s.begin(), s.end());
+        longest = std::max(longest, pc.len);
+    }
+    d->node_bytes = longest + 1;
+    // the label pieces right behind the B2cTok table (B2cPiece)
+    const size_t tok_bytes = sizeof(B2cTok) * n_labels;
+    if (d->d_toks.ensure(tok_bytes + pieces.size())) return B2C_E_NOMEM;
+    CUDA_OK(cudaMemcpy(d->d_toks.p, d->toks.data(), tok_bytes, cudaMemcpyHostToDevice));
+    CUDA_OK(cudaMemcpy(d->d_toks.as<u8>() + tok_bytes, pieces.data(), pieces.size(), cudaMemcpyHostToDevice));
     if (lm) {
         int rc = b2c_lm_upload(lm, device);
         if (rc) return rc;
@@ -1745,6 +1818,7 @@ static int make_params(b2c_decoder* d, Call& c) {
     B2cParams& P = c.P;
     P.V = c.g.V; P.is_bpe = d->is_bpe; P.has_dup_labels = d->has_dup_labels;
     P.beam_width = c.g.beam_width; P.prune_history = o->prune_history ? 1 : 0; P.out_beams = c.OB; P.narrow_chain = c.text_only ? 1 : 0;
+    P.text_node_bytes = c.text_only ? d->node_bytes : 0;
     P.prune_logp = o->beam_prune_logp; P.token_min_logp = o->token_min_logp;
     P.bucket_scale = b2c_bucket_scale(o->beam_prune_logp);
     P.kflags = c.k.no_single ? B2C_FL_NO_SINGLE : 0;
@@ -1787,9 +1861,18 @@ static int size_buffers(b2c_decoder* d, Call& c) {
     g.smem_budget = static_cast<u32>(std::min<size_t>(d->smem_optin, 200 * 1024));
     c.out = OutLayout(n, c.OB, g.n_lm, g.streaming);
     c.tok_bytes = 4ull * c.OB * (g.total_frames + n); c.frm_bytes = 2 * c.tok_bytes;
-    if (d->d_out_small.ensure(c.out.bytes) || d->h_out_small.ensure(c.out.bytes) || d->d_out_toks.ensure(c.tok_bytes) ||
-        d->h_out_toks.ensure(c.tok_bytes) || d->d_out_frames.ensure(c.frm_bytes) || d->h_out_frames.ensure(c.frm_bytes))
+    if (d->d_out_small.ensure(c.out.bytes) || d->h_out_small.ensure(c.out.bytes)) return B2C_E_NOMEM;
+    if (c.text_only) {
+        // a transcript adds at most node_bytes per backtrack node, T + 1 nodes per beam; the joined copy adds a '\0' per
+        // slot.  What the token chains would have cost is read back with the small outputs, the rest (long pieces) after.
+        const u64 text_bytes = static_cast<u64>(c.OB) * (g.total_frames + n) * d->node_bytes;
+        c.join_bytes = 8 + text_bytes + static_cast<u64>(c.OB) * n;
+        c.join_first = std::min(c.join_bytes, c.tok_bytes);
+        if (d->d_text.ensure(text_bytes) || d->d_join.ensure(c.join_bytes) || d->h_join.ensure(c.join_bytes)) return B2C_E_NOMEM;
+    } else if (d->d_out_toks.ensure(c.tok_bytes) || d->h_out_toks.ensure(c.tok_bytes) || d->d_out_frames.ensure(c.frm_bytes) ||
+               d->h_out_frames.ensure(c.frm_bytes)) {
         return B2C_E_NOMEM;
+    }
     if (c.opts->lm_start_states && d->d_states.ensure(sizeof(B2cLmState) * static_cast<u64>(n) * g.n_lm)) return B2C_E_NOMEM;
     return 0;
 }
@@ -1955,7 +2038,7 @@ static int fill_beam_args(b2c_decoder* d, Call& c) {
     const OutViews o = c.out.at(d->d_out_small.as<u8>());
     BA.out_nbeams = o.nbeams; BA.out_status = o.status; BA.out_scores = o.scores; BA.out_ntok = o.ntok; BA.out_nwords = o.nwords;
     BA.out_states = o.states; BA.out_aux = o.aux; BA.out_states_x = o.states_x;
-    BA.out_toks = d->d_out_toks.as<u32>(); BA.out_frames = d->d_out_frames.as<int>();
+    BA.out_toks = c.text_only ? d->d_text.as<u32>() : d->d_out_toks.as<u32>(); BA.out_frames = d->d_out_frames.as<int>();
     if (d->d_mstats.ensure(64)) return B2C_E_NOMEM;
     CUDA_OK(cudaMemsetAsync(d->d_mstats.p, 0, 64, d->stream));
     BA.m_stats = d->d_mstats.as<u32>();
@@ -2121,10 +2204,43 @@ static int enqueue_plain(b2c_decoder* d, Call& c) {
     return 0;
 }
 
-static int read_outputs(b2c_decoder* d, const Call& c, bool frames) {
+// text-only calls: the transcripts of the beam launches, joined (b2c_join_block)
+static int launch_join(b2c_decoder* d, const Call& c) {
+    const OutViews o = c.out.at(d->d_out_small.as<u8>());
+    const B2cJoinArgs J{c.g.n_utts, c.OB, d->node_bytes, 0u, o.nbeams, o.ntok, c.PA.frame_off, c.PA.T, d->d_text.as<u8>(), d->d_join.as<u8>()};
+    const int grid = (c.g.n_utts * c.OB + B2C_JOIN_TILE - 1) / B2C_JOIN_TILE;
+    d->tm.launches += 1;
+#ifdef B2C_HOSTSIM
+    std::unique_ptr<B2cJoinShared> sh(new B2cJoinShared());
+    for (int b = 0; b < grid; ++b) b2c_join_block(J, b, sh.get());
+#else
+    b2c_join_kernel<<<grid, B2C_JOIN_THREADS, 0, d->stream>>>(J);
+    CUDA_OK(cudaGetLastError());
+#endif
+    return 0;
+}
+
+static int read_outputs(b2c_decoder* d, const Call& c) {
     CUDA_OK(cudaMemcpyAsync(d->h_out_small.p, d->d_out_small.p, c.out.bytes, cudaMemcpyDeviceToHost, d->stream));
+    if (c.text_only) {
+        B2C_TRY(launch_join(d, c));
+        CUDA_OK(cudaMemcpyAsync(d->h_join.p, d->d_join.p, c.join_first, cudaMemcpyDeviceToHost, d->stream));
+        return 0;
+    }
     CUDA_OK(cudaMemcpyAsync(d->h_out_toks.p, d->d_out_toks.p, c.tok_bytes, cudaMemcpyDeviceToHost, d->stream));
-    if (frames) CUDA_OK(cudaMemcpyAsync(d->h_out_frames.p, d->d_out_frames.p, c.frm_bytes, cudaMemcpyDeviceToHost, d->stream));
+    CUDA_OK(cudaMemcpyAsync(d->h_out_frames.p, d->d_out_frames.p, c.frm_bytes, cudaMemcpyDeviceToHost, d->stream));
+    return 0;
+}
+
+// text-only calls, once the last beam launch and its join are done: the joined transcripts past what read_outputs copied
+static int read_text_rest(b2c_decoder* d, const Call& c) {
+    if (!c.text_only) return 0;
+    const u64 need = 8 + *d->h_join.as<u64>();
+    if (need <= c.join_first) return 0;
+    CUDA_OK(cudaMemcpyAsync(d->h_join.as<u8>() + c.join_first, d->d_join.as<u8>() + c.join_first, need - c.join_first,
+                            cudaMemcpyDeviceToHost, d->stream));
+    CUDA_OK(cudaStreamSynchronize(d->stream));
+    d->tm.d2h_bytes += static_cast<long long>(need - c.join_first);
     return 0;
 }
 
@@ -2132,7 +2248,7 @@ static int read_outputs(b2c_decoder* d, const Call& c, bool frames) {
 static int read_back(b2c_decoder* d, Call& c) {
     const int n = c.g.n_utts;
     cudaStream_t st = d->stream;
-    B2C_TRY(read_outputs(d, c, !c.text_only));
+    B2C_TRY(read_outputs(d, c));
     if (d->h_mstats.ensure(64)) return B2C_E_NOMEM;
     CUDA_OK(cudaMemcpyAsync(d->h_mstats.p, d->d_mstats.p, 64, cudaMemcpyDeviceToHost, st));
     // selected-token totals (b2c_timings_t.tokens); a plain call already copied them for the launch plan
@@ -2147,7 +2263,7 @@ static int read_back(b2c_decoder* d, Call& c) {
         // the streaming stage of a later chunk never got to run beside the beam kernel
         for (int i = 0; i < n; ++i) if (status[i] & B2C_ERR_GATE) { d->pipe_refused = true; return B2C_E_RETRY_PLAIN; }
     }
-    d->tm.d2h_bytes += static_cast<long long>(c.out.bytes + c.tok_bytes + (c.text_only ? 0 : c.frm_bytes) + 8ull * n + 32);
+    d->tm.d2h_bytes += static_cast<long long>(c.out.bytes + (c.text_only ? c.join_first : c.tok_bytes + c.frm_bytes) + 8ull * n + 32);
     const u32* ms = d->h_mstats.as<u32>();
     d->hint_valid = true;
     d->hint_beam = c.g.beam_width; d->hint_lm = c.any_lm ? 1 : 0; d->hint_hot = c.any_hot ? 1 : 0; d->hint_prune = c.P.prune_history;
@@ -2180,7 +2296,7 @@ static int retry_failed(b2c_decoder* d, Call& c) {
     c.BA.L = ln.L; c.BA.n_utts = ln.count; c.BA.order = c.d_ord() + n; c.BA.next = c.d_next() + 15; c.BA.gws = d->d_ws.as<u8>();
     c.BA.chunk_t1 = 0;
     B2C_TRY(launch_beam(d, c.BA, ln, st, false));
-    B2C_TRY(read_outputs(d, c, true));
+    B2C_TRY(read_outputs(d, c));
     CUDA_OK(cudaStreamSynchronize(st));
     for (int i : failed)
         if (status[i] != B2C_OK) return fail(B2C_E_INTERNAL, "beam kernel workspace overflow (status " + std::to_string(status[i]) + ")");
@@ -2251,8 +2367,7 @@ static void assemble_range(const b2c_decoder* d, const Call& c, b2c_result* res,
             br.st = h.states[k];
             if (h.states_x && c.utt_models[u] > 1)
                 br.stx.assign(h.states_x + k * (n_lm - 1), h.states_x + k * (n_lm - 1) + (c.utt_models[u] - 1));
-            if (c.text_only) assemble_text(d, h_toks + base + r * stride, h.ntok[k], br);
-            else assemble_beam(d, h_toks + base + r * stride, h.ntok[k], h_frames + 2 * (base + r * stride), h.nwords[k], br);
+            assemble_beam(d, h_toks + base + r * stride, h.ntok[k], h_frames + 2 * (base + r * stride), h.nwords[k], br);
             if (h.aux) {
                 const u32* tk = h_toks + base + r * stride;
                 br.raw.resize(static_cast<size_t>(h.ntok[k]));
@@ -2287,6 +2402,15 @@ static void assemble(b2c_decoder* d, const Call& c, b2c_result* res) {
     const int n = c.g.n_utts;
     res->n_models = c.g.n_lm;
     res->streaming = c.g.streaming;
+    if (c.text_only) {
+        const u8* h_small = d->h_out_small.as<u8>();
+        res->text_only = true;
+        res->OB = c.OB;
+        res->out = c.out;
+        res->small.assign(h_small, h_small + c.out.bytes);
+        res->texts.assign(d->h_join.as<char>() + 8, *d->h_join.as<u64>());
+        return;
+    }
     const u64 work = (c.g.total_frames + static_cast<u64>(n)) * static_cast<u64>(c.OB);
     int n_thr = static_cast<int>(std::min<u64>(std::min<u64>(8, std::max(1u, std::thread::hardware_concurrency())), work / 32768));
     n_thr = std::min(n_thr, n);
@@ -2301,7 +2425,8 @@ static void assemble(b2c_decoder* d, const Call& c, b2c_result* res) {
 }
 
 static int decode_batch_locked(b2c_decoder_t* d, const void* const* logits, const int32_t* T, int n_utts, int dtype, int is_device,
-                               const b2c_decode_opts_t* opts, b2c_result_t** out, bool allow_pipe) {
+                               const b2c_decode_opts_t* opts, b2c_result_t** out, bool allow_pipe,
+                               std::chrono::steady_clock::time_point entry) {
     if (dtype < B2C_DTYPE_F32 || dtype > B2C_DTYPE_BF16) return fail(B2C_E_ARG, "dtype must be one of B2C_DTYPE_F32 / F64 / F16 / BF16");
     Call c(d, logits, T, n_utts, dtype, is_device, opts, allow_pipe);
     d->last_T.clear();
@@ -2326,12 +2451,14 @@ static int decode_batch_locked(b2c_decoder_t* d, const void* const* logits, cons
     B2C_TRY(enqueue_plain(d, c));
     B2C_TRY(read_back(d, c));
     B2C_TRY(retry_failed(d, c));
+    B2C_TRY(read_text_rest(d, c));
     B2C_TRY(record_timings(d, c));
     assemble(d, c, res.get());
     c.hp.mark(4);                                 // statistics read-back, result assembly
     if (c.k.host_prof)
-        std::fprintf(stderr, "[b2c host ms] enqueue=%.3f wait_prepare=%.3f plan=%.3f wait_beam=%.3f assemble=%.3f hotwords=%.3f lm_sets=%.3f\n",
-                     c.hp.ms[0], c.hp.ms[1], c.hp.ms[2], c.hp.ms[3], c.hp.ms[4], c.hp.ms[5], c.hp.ms[6]);
+        std::fprintf(stderr, "[b2c host ms] enqueue=%.3f wait_prepare=%.3f plan=%.3f wait_beam=%.3f assemble=%.3f hotwords=%.3f lm_sets=%.3f "
+                     "library=%.3f\n", c.hp.ms[0], c.hp.ms[1], c.hp.ms[2], c.hp.ms[3], c.hp.ms[4], c.hp.ms[5], c.hp.ms[6],
+                     std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - entry).count());
     *out = res.release();
     return 0;
 }
@@ -2339,21 +2466,56 @@ static int decode_batch_locked(b2c_decoder_t* d, const void* const* logits, cons
 int b2c_decode_batch(b2c_decoder_t* d, const void* const* logits, const int32_t* T, int n_utts, int dtype, int is_device,
                      const b2c_decode_opts_t* opts, b2c_result_t** out) {
     if (!d || !opts || !out || n_utts < 0 || (n_utts > 0 && (!logits || !T))) return fail(B2C_E_ARG, "null argument");
+    // B200CTC_HOST_PROFILE: library= is the time from here to the return, a pipelined attempt that is redone included
+    const auto entry = std::chrono::steady_clock::now();
     std::lock_guard<std::mutex> call_lock(d->call_mu);      // one call at a time per handle (any number of threads may call)
-    int rc = decode_batch_locked(d, logits, T, n_utts, dtype, is_device, opts, out, true);
+    int rc = decode_batch_locked(d, logits, T, n_utts, dtype, is_device, opts, out, true, entry);
     // a pipelined attempt that could not be planned, or that met probability input (decided after the fact): plain call
-    if (rc == B2C_E_RETRY_PLAIN) rc = decode_batch_locked(d, logits, T, n_utts, dtype, is_device, opts, out, false);
+    if (rc == B2C_E_RETRY_PLAIN) rc = decode_batch_locked(d, logits, T, n_utts, dtype, is_device, opts, out, false, entry);
     return rc;
 }
 
 // ---- results ------------------------------------------------------------------------------
 void b2c_result_free(b2c_result_t* r) { delete r; }
 int b2c_result_n_utts(const b2c_result_t* r) { return r ? static_cast<int>(r->utts.size()) : 0; }
-int b2c_result_n_beams(const b2c_result_t* r, int u) { return static_cast<int>(r->utts[u].size()); }
-const char* b2c_result_text(const b2c_result_t* r, int u, int b) { return r->utts[u][b].text.c_str(); }
+// the beams of a result; a text-only result builds them from its joined transcripts and small outputs on first use
+static const std::vector<std::vector<BeamRes>>& beams_of(const b2c_result* r) {
+    if (!r->text_only) return r->utts;
+    std::call_once(r->built, [r]() {
+        const OutViews h = r->out.at(const_cast<u8*>(r->small.data()));
+        const int n_lm = r->n_models;
+        size_t p = 0;
+        for (size_t u = 0; u < r->utts.size(); ++u) {
+            const int nb = h.nbeams[u];
+            r->utts[u].resize(static_cast<size_t>(nb));
+            for (int b = 0; b < nb; ++b) {
+                BeamRes& br = r->utts[u][b];
+                const u64 k = static_cast<u64>(u) * r->OB + b;
+                br.logit = h.scores[2 * k];
+                br.lm = h.scores[2 * k + 1];
+                br.st = h.states[k];
+                if (h.states_x && r->utt_models[u] > 1)
+                    br.stx.assign(h.states_x + k * (n_lm - 1), h.states_x + k * (n_lm - 1) + (r->utt_models[u] - 1));
+                const size_t q = r->texts.find('\0', p);
+                br.text.assign(r->texts, p, q - p);
+                p = q + 1;
+            }
+            if (nb == 0) p = r->texts.find('\0', p) + 1;      // the utterance's empty entry
+        }
+    });
+    return r->utts;
+}
+int b2c_result_n_beams(const b2c_result_t* r, int u) { return static_cast<int>(beams_of(r)[u].size()); }
+const char* b2c_result_text(const b2c_result_t* r, int u, int b) { return beams_of(r)[u][b].text.c_str(); }
 int b2c_result_top_texts(b2c_result_t* r, const char** data, size_t* size) {
     if (!r || !data || !size) return fail(B2C_E_ARG, "null argument");
+    if (r->text_only && r->OB == 1) {       // one entry per utterance: the buffer as the device joined it
+        *data = r->texts.data();
+        *size = r->texts.size();
+        return 0;
+    }
     if (!r->joined_built) {
+        beams_of(r);
         size_t total = 0;
         for (const auto& u : r->utts) total += (u.empty() ? 0 : u[0].text.size()) + 1;
         r->joined.reserve(total);
@@ -2370,6 +2532,7 @@ int b2c_result_top_texts(b2c_result_t* r, const char** data, size_t* size) {
 int b2c_result_packed(b2c_result_t* r, b2c_packed_t* out) {
     if (!r || !out) return fail(B2C_E_ARG, "null argument");
     if (!r->packed_built) {
+        beams_of(r);
         size_t nb = 0, nw = 0, nt = 0;
         for (const auto& u : r->utts)
             for (const auto& b : u) { ++nb; nw += b.frames.size() / 2; nt += b.text.size() + 1; }
@@ -2429,34 +2592,34 @@ int b2c_result_packed(b2c_result_t* r, b2c_packed_t* out) {
     out->stream_boundary = r->streaming ? r->pk_boundary.data() : nullptr;
     return 0;
 }
-double b2c_result_logit_score(const b2c_result_t* r, int u, int b) { return r->utts[u][b].logit; }
-double b2c_result_lm_score(const b2c_result_t* r, int u, int b) { return r->utts[u][b].lm; }
-int b2c_result_n_words(const b2c_result_t* r, int u, int b) { return static_cast<int>(r->utts[u][b].words.size()); }
-const char* b2c_result_word(const b2c_result_t* r, int u, int b, int w) { return r->utts[u][b].words[w].c_str(); }
-const int32_t* b2c_result_frames(const b2c_result_t* r, int u, int b) { return r->utts[u][b].frames.data(); }
+double b2c_result_logit_score(const b2c_result_t* r, int u, int b) { return beams_of(r)[u][b].logit; }
+double b2c_result_lm_score(const b2c_result_t* r, int u, int b) { return beams_of(r)[u][b].lm; }
+int b2c_result_n_words(const b2c_result_t* r, int u, int b) { return static_cast<int>(beams_of(r)[u][b].words.size()); }
+const char* b2c_result_word(const b2c_result_t* r, int u, int b, int w) { return beams_of(r)[u][b].words[w].c_str(); }
+const int32_t* b2c_result_frames(const b2c_result_t* r, int u, int b) { return beams_of(r)[u][b].frames.data(); }
 int b2c_result_lm_state(const b2c_result_t* r, int u, int b, b2c_lm_state_t* out) {
     if (!r->has_lm || r->utt_models[u] == 0) return 0;
-    from_internal(r->utts[u][b].st, out);
+    from_internal(beams_of(r)[u][b].st, out);
     return 1;
 }
 int b2c_result_lm_state_at(const b2c_result_t* r, int u, int b, int lm_index, b2c_lm_state_t* out) {
     if (!r->has_lm || r->utt_models[u] == 0) return 0;
-    const BeamRes& br = r->utts[u][b];
+    const BeamRes& br = beams_of(r)[u][b];
     if (lm_index == 0) { from_internal(br.st, out); return 1; }
     if (lm_index < 0 || lm_index > static_cast<int>(br.stx.size())) return 0;
     from_internal(br.stx[lm_index - 1], out);
     return 1;
 }
 int b2c_result_stream_beam(const b2c_result_t* r, int u, int b, int32_t aux[4], const uint32_t** toks, int* n_toks) {
-    if (!r || u < 0 || u >= static_cast<int>(r->utts.size()) || b < 0 || b >= static_cast<int>(r->utts[u].size()))
+    if (!r || u < 0 || u >= static_cast<int>(r->utts.size()) || b < 0 || b >= static_cast<int>(beams_of(r)[u].size()))
         return fail(B2C_E_ARG, "no such beam");
-    const BeamRes& br = r->utts[u][b];
+    const BeamRes& br = beams_of(r)[u][b];
     for (int q = 0; q < 4; ++q) aux[q] = br.aux[q];
     *toks = br.raw.data();
     *n_toks = static_cast<int>(br.raw.size());
     return 0;
 }
-int b2c_result_n_frames(const b2c_result_t* r, int u, int b) { return static_cast<int>(r->utts[u][b].frames.size() / 2); }
+int b2c_result_n_frames(const b2c_result_t* r, int u, int b) { return static_cast<int>(beams_of(r)[u][b].frames.size() / 2); }
 int b2c_hash_utf8(const char* s, uint64_t* hash, uint32_t* n_chars) {
     if (!s || !hash || !n_chars) return fail(B2C_E_ARG, "null argument");
     const size_t n = std::strlen(s);

@@ -1219,7 +1219,41 @@ struct B2cOut {              // per-utterance output views (HBM)
     int* aux;                // [out_beams][4] streaming: input beam the output descends from (-1: none), canonical
                              // token of last_char (-1: None), partial_frames; nullptr outside streaming calls
     u32 stride;              // T + 1
+    // text-only calls (P.narrow_chain): no toks / frames / n_words; the transcript of beam r ends at the end of its
+    // region [r, r + 1) * stride * P.text_node_bytes of `text`, its length in bytes goes to n_tok[r]
+    u8* text;
 };
+
+// The transcript of one beam, walked from its newest node and written backwards so that it ends at `end`; the same bytes
+// as joining the beam's non-empty words with one space (a word: the clean piece of its BPE node, if any, then its CONT
+// labels; SPACE and BPE nodes end the word before them).  Returns its length.  Out of line: finalize only.
+B2C_HDN u32 b2c_walk_text(const B2cChain* chain, u32 node, u32 max_nodes, const B2cPiece* pieces, u8* end) {
+    const u8* bytes = reinterpret_cast<const u8*>(pieces);
+    const u64* nodes = reinterpret_cast<const u64*>(chain);      // the 8-byte nodes of b2c_chain_store
+    u8* p = end;
+    bool open = false;           // the word being written (its last bytes first) has a byte
+    u64 v = node != B2C_NONE_U32 ? nodes[node] : 0;
+    for (u32 nt = 0; node != B2C_NONE_U32 && nt < max_nodes; ++nt) {
+        const u32 parent = static_cast<u32>(v), tok = static_cast<u16>(v >> 32), kind = static_cast<u8>(v >> 48);
+        if (kind == B2C_CK_ROOT) break;
+        // the parent's load goes out before this node's piece is copied: the chase of parent pointers (HBM latency
+        // per node) stays the only serial chain of the walk
+        const u64 pv = parent != B2C_NONE_U32 ? nodes[parent] : 0;
+        if (kind != B2C_CK_SPACE) {
+            const B2cPiece pc = pieces[2u * tok + (kind == B2C_CK_BPE ? 1u : 0u)];
+            if (pc.len) {
+                if (!open && p != end) *--p = ' ';      // a later word is written already
+                p -= pc.len;
+                for (u32 i = 0; i < pc.len; ++i) p[i] = bytes[pc.off + i];
+                open = true;
+            }
+        }
+        if (kind != B2C_CK_CONT) open = false;
+        node = parent;
+        v = pv;
+    }
+    return static_cast<u32>(end - p);
+}
 
 B2C_HDN void b2c_finalize(B2cParams P, B2cWork W, B2cOut O, int fin_mode) {
     const bool keep = fin_mode == B2C_FIN_KEEP;
@@ -1318,6 +1352,12 @@ B2C_HDN void b2c_finalize(B2cParams P, B2cWork W, B2cOut O, int fin_mode) {
             }
         }
         O.states[r] = st;
+        if (P.narrow_chain) {
+            u8* end = O.text + (static_cast<u64>(r) + 1) * O.stride * P.text_node_bytes;
+            const B2cPiece* pieces = reinterpret_cast<const B2cPiece*>(P.toks + P.V);
+            O.n_tok[r] = static_cast<int>(b2c_walk_text(W.chain, cur.chain[last], O.stride, pieces, end));
+            continue;
+        }
         u32* toks = O.toks + static_cast<u64>(r) * O.stride;
         int* frames = O.frames + static_cast<u64>(r) * O.stride * 2;
         u32 nt = 0, nw = 0;

@@ -1895,6 +1895,7 @@ B2C_HD void b2c_beam_block_fast(const B2cBeamArgs& A, int slot_cta, u8* smem) {
         O.states = A.out_states + static_cast<u64>(u) * ob;
         O.aux = nullptr;
         O.states_x = nullptr;
+        O.text = reinterpret_cast<u8*>(A.out_toks) + ob * (f0 + static_cast<u64>(u)) * A.P.text_node_bytes;
         b2c_fast_compact<CAP, LT>(&S, par);
         par ^= 1;
         {

@@ -124,6 +124,10 @@ struct B2cTok {          // 32 bytes, one per label
     u16 canon;           // first token id with the same label string (string compare semantics)
     u16 flags;
 };
+// Text-only calls write their transcripts on the device from one blob uploaded at decoder creation right behind the
+// [V] B2cTok table (at P.toks + V): [2V] pieces (2 tok: the label, read for CONT nodes; 2 tok + 1: the label without
+// U+2581, read for BPE nodes), then the bytes they point at (`off` counts from the start of the blob).
+struct B2cPiece { u32 off, len; };
 
 // ---------------------------------------------------------------------------------------
 // n-gram model, flattened (KenLM probing-model semantics: float32 log10 prob / backoff,
@@ -206,7 +210,7 @@ struct B2cParams {
                                // copied into every out-of-line call of the hot kernels)
     const u32* utt_lm;         // [n_utts] set of each utterance, copied into B2cScalars::lm_set by b2c_utt_begin
     int kflags;                // extra B2C_FL_* mode bits set by the host (B2C_FL_NO_SINGLE: B200CTC_NO_SINGLE_STEP)
-    int pad_params;
+    u32 text_node_bytes;       // text-only calls: the most bytes one backtrack node adds to a transcript (longest piece + 1)
 };
 
 // ---------------------------------------------------------------------------------------
